@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the VINS-Mono hot path (feature tracker + sliding-window BA) on B200.
+"""bench.py — frames/sec of the VINS-Mono hot path (feature tracker + sliding-window BA) on H100.
 
 A "step" is one published (10 Hz) frame of one sequence, fully processed: the two 752x480 camera images that
 arrive in that interval go through FeatureTracker::readImage (the second one publishes), the ~20 IMU samples
@@ -13,6 +13,7 @@ Workloads (BASELINE.json configs):
   --config c3       emit the configs[2] line as the main line on one GPU
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            our CUDA path
+  python bench.py ... --dump-outputs DIR                          also writes the last timed step's outputs as DIR/<name>.npy
   python bench.py --impl reference ...                            the CPU path: cv2 (OpenCV) tracker twin + oracle estimator
 Under torchrun (N > 1) rank 0 prints ONE JSON line.
 """
@@ -259,6 +260,7 @@ def run_ours_pass(seq, ts, imgs, imu, n_init, warmup, steps, device, host_images
 
     stage = Serial() if profile else TwoStage(produce, n_init + warmup, n_pub)
     pubs, first_msg, n_timed, started = 0, True, 0, False
+    last_msg = None
     while pubs < n_pub:
         timed = pubs >= n_init + warmup
         if timed and not started:
@@ -283,6 +285,7 @@ def run_ours_pass(seq, ts, imgs, imu, n_init, warmup, steps, device, host_images
             step_d2h += b
         if timed:
             n_timed += 1
+            last_msg = (ids, d)
             launches += step_launch
             h2d += step_h2d
             d2h += step_d2h
@@ -295,6 +298,9 @@ def run_ours_pass(seq, ts, imgs, imu, n_init, warmup, steps, device, host_images
     stage.go()
     times = [region_ms / max(n_timed, 1)] * n_timed if started else []
     out = dict(times=times, launches=launches, h2d=h2d, d2h=d2h, traj_t=traj_t, traj_p=traj_p, info=est.info())
+    if last_msg is not None:  # what a caller holds after the last timed step: the feature message and the window states
+        st, td = est.states()
+        out["last"] = {"feature_ids": last_msg[0], "features_xyz_uv_vel": last_msg[1], "window_states": st, "td": np.array([td])}
     if profile:
         out["trk_k"], out["est_k"] = trk.kernel_times(), est.kernel_times()
     trk.close()
@@ -375,11 +381,13 @@ def run_batch_pass(inputs, n_seq, n_init, warmup, steps, device, host_images=Fal
     after = [ses.stats(k) for k in range(n_seq)]
     trajs = [ses.trajectory(k) for k in range(n_seq)]
     infos = [m.info() for m in eb.members]
+    member_states = [m.states() for m in eb.members]
     out = dict(frames=frames, region_ms=region_ms, fps=frames / (region_ms / 1e3) if region_ms else 0.0,
                launches=sum(a_["launches"] - b_["launches"] for a_, b_ in zip(after, before)),
                h2d=sum(a_["h2d"] - b_["h2d"] for a_, b_ in zip(after, before)),
                d2h=sum(a_["d2h"] - b_["d2h"] for a_, b_ in zip(after, before)), trajs=trajs, infos=infos)
     out["est_groups"] = eb.groups()
+    out["last"] = {"window_states": np.stack([st for st, _ in member_states]), "td": np.array([td for _, td in member_states])}
     if profile:
         out["trk_k"], out["est_k"] = tb.kernel_times(), eb.kernel_times()
     ses.close()
@@ -544,10 +552,17 @@ def roofline_object(kt, n_solves, n_images, units_per_launch, peak, peaks_found,
     dk = per_kernel[dominant]
     return {"bound": "hbm", "kernel": dominant, "achieved": dk["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": dk["frac"],
             "traffic": traffic,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst copy)" if peaks_found else "fallback 6650 GB/s",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst copy)" if peaks_found else "fallback 3350 GB/s (H100 SXM data sheet)",
             "algorithmic_bytes_per_launch": dk["algorithmic_bytes_per_launch"], "avg_launch_us": dk["avg_us"],
             "profiled_solves": n_solves, "profiled_images": n_images, "sequences_per_launch": units_per_launch,
             "note": note, "kernels": per_kernel}
+
+
+def dump_outputs(directory, arrays):
+    """Writes each array as directory/<name>.npy in float64 (ids included: they are exact in float64)."""
+    os.makedirs(directory, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), np.asarray(arr, np.float64))
 
 
 def main():
@@ -564,7 +579,13 @@ def main():
     ap.add_argument("--seqs-per-gpu", type=int, default=SEQS_PER_GPU, help="members of the batched workload (configs[2]/[4])")
     ap.add_argument("--distinct", type=int, default=16, help="distinct rendered sequences behind the batch members")
     ap.add_argument("--no-c3", action="store_true", help="skip the configs[2] object of the single-GPU line")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy (float64): "
+                         "the feature message and window states of the headline sequence, the window states of every batch member "
+                         "(c3_*)")
     a = ap.parse_args()
+    if a.dump_outputs and a.impl != "b200":
+        ap.error("--dump-outputs applies to the CUDA path (--impl b200)")
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     warmup = max(a.warmup, 3) if a.impl == "b200" else a.warmup
     global INIT_PUBS, WORKLOAD
@@ -644,12 +665,12 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))  # H100 SXM data sheet HBM3 bandwidth
 
     # frames are rendered (fork pool) before this process touches CUDA; the CPU-baseline sample needs a longer sequence
     cpu_frames = max(a.steps, a.cpu_frames) if (not a.no_cpu_baseline and world == 1 and not batched) else a.steps
     want_c3 = (batched or not a.no_c3)
-    c3_steps = min(a.steps, 20)
+    c3_steps = a.steps
     batch_inputs = None
     if want_c3:
         first_seed = 100 + shard.sequences_of_rank(rank, world, S)[0]
@@ -672,7 +693,7 @@ def main():
         if os.environ.get("NCCL_DEBUG", "VERSION").upper() == "VERSION":
             os.environ["NCCL_DEBUG"] = "WARN"  # keeps NCCL's version banner off stdout: rank 0 prints ONE JSON line
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local}"))
-    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=f"cuda:{local}")  # 256 MB > 126 MB L2
+    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=f"cuda:{local}")  # 256 MB > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize(local)
@@ -753,6 +774,8 @@ def main():
                 "gpu_launches": int(launches.item()), "roofline": obj.get("roofline"), "cpu_baseline": None, "clocks": obj["clocks"],
                 "parity": obj.get("parity"), "ate_rmse_m": obj["ate_rmse_m_mean"],
             }))
+            if a.dump_outputs:
+                dump_outputs(a.dump_outputs, {"c3_" + k: v for k, v in rb["last"].items()})
         if world > 1:
             dist.destroy_process_group()
         return
@@ -839,6 +862,11 @@ def main():
         "ate_rel_diff": (abs(ate_same - ate_ref) / ate_ref) if ate_ref else None,
         "solver": res_dev["info"], "self_init": self_init_check(local) if rank == 0 else None,
     }))
+    if a.dump_outputs:
+        arrays = dict(res_dev.get("last", {}))
+        if c3 is not None:
+            arrays.update({"c3_" + k: v for k, v in rb["last"].items()})
+        dump_outputs(a.dump_outputs, arrays)
 
 
 if __name__ == "__main__":

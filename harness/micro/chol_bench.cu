@@ -1,5 +1,5 @@
 // Phase timing of the single-CTA packed Cholesky / triangular solves of ba_step_kernel on a synthetic SPD matrix.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I include -I vins_mono_b200/csrc -o harness/micro/chol_bench harness/micro/chol_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I include -I vins_mono_b200/csrc -o harness/micro/chol_bench harness/micro/chol_bench.cu
 #define CHOL_PROF 1
 #include "../../vins_mono_b200/csrc/ba_kernels.cu"
 #include <cstdio>

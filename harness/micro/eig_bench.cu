@@ -1,6 +1,6 @@
 // Phase timing of the single-CTA symmetric eigen-solver (vins_mono_b200/csrc/sym_eig.h) on a real marginalisation
 // prior (harness/micro/prior75.bin: the 75x75 Schur complement A' of a steady-state frame, dumped from the CPU twin).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o harness/micro/eig_bench harness/micro/eig_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o harness/micro/eig_bench harness/micro/eig_bench.cu
 #define SE_PROF 1
 #include "../../vins_mono_b200/csrc/prior_floor.h"
 #include <cstdio>

@@ -1,5 +1,5 @@
 // Latency microbenchmarks (dependent chains, one warp) used to size the serial sections of the single-CTA solvers.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o harness/micro/lat harness/micro/lat.cu ; run on the GPU box.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o harness/micro/lat harness/micro/lat.cu ; run on an H100.
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N 2048

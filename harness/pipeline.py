@@ -6,13 +6,16 @@ from __future__ import annotations
 
 import hashlib
 import os
+import tempfile
 
 import numpy as np
 
 from . import synth
 
 
-def cached_images(seq: synth.Sequence, n: int, cache_dir="/tmp/vinsb200_cache"):
+def cached_images(seq: synth.Sequence, n: int, cache_dir=None):
+    # rendered frames are cached per user outside the tree (the tree may be read-only, /tmp is shared)
+    cache_dir = cache_dir or os.path.join(tempfile.gettempdir(), f"vinsb200_cache_{os.getuid()}")
     os.makedirs(cache_dir, exist_ok=True)
     key = hashlib.sha1(f"{seq.seed}-{seq.rows}x{seq.cols}-{seq.pixel_noise}-{seq.cam_hz}-{n}-v2".encode()).hexdigest()[:16]
     path = os.path.join(cache_dir, key + ".npy")
@@ -20,7 +23,10 @@ def cached_images(seq: synth.Sequence, n: int, cache_dir="/tmp/vinsb200_cache"):
     if os.path.exists(path):
         return ts, np.load(path, mmap_mode="r")
     _, imgs = seq.images(n)
-    np.save(path, imgs)
+    tmp = f"{path}.{os.getpid()}.tmp"
+    with open(tmp, "wb") as f:
+        np.save(f, imgs)
+    os.replace(tmp, path)  # concurrent readers never see a partial file
     return ts, imgs
 
 

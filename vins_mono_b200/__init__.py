@@ -1,6 +1,6 @@
-"""vins_mono_b200 — B200-native hot paths of VINS-Mono behind a C ABI (include/vinsb200/*.h).
+"""vins_mono_b200 — H100-native (sm_90a) hot paths of VINS-Mono behind a C ABI (include/vinsb200/*.h).
 
-The product is lib/libvinsb200.so (hand-written CUDA for sm_100a + host glue); this package is a thin
+The product is lib/libvinsb200.so (hand-written CUDA for sm_90a + host glue); this package is a thin
 ctypes mirror of the reference's host classes for tests and benchmarks.  There is no CPU fallback:
 loading fails loudly when the library is missing, creating a tracker fails when no CUDA device exists.
 """

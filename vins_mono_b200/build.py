@@ -1,4 +1,4 @@
-"""Builds libvinsb200.so (CUDA kernels + C ABI + host glue) in-tree for sm_100a with nvcc."""
+"""Builds libvinsb200.so (CUDA kernels + C ABI + host glue) in-tree for sm_90a (H100) with nvcc."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,8 @@ LIB = os.path.join(HERE, "lib", "libvinsb200.so")
 
 # The front end must reproduce OpenCV's float arithmetic bit for bit: no FMA contraction there.  The back end is
 # double precision checked to a tolerance, so its kernels (ba_*.cu) keep nvcc's default contraction (DFMA).
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-O2", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
@@ -51,7 +52,7 @@ def build(force=False, verbose=False):
             raise RuntimeError(f"nvcc failed for {src}:\n{out}")
         if verbose and out.strip():
             print(out)
-    subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB, *objs])
+    subprocess.check_call(["nvcc", *ARCH, "-shared", "-o", LIB, *objs])
     return LIB
 
 

@@ -1,4 +1,4 @@
-// Sliding-window BA kernels for sm_100a (SURVEY.md §8 rows b1, b5-b11, b13), float64.
+// Sliding-window BA kernels for sm_90a (SURVEY.md §8 rows b1, b5-b11, b13), float64.
 //
 //   preint_push_kernel    IntegrationBase::propagate / midPointIntegration     integration_base.h:54-158
 //   sqrt_info_kernel      LLT(covariance^-1).matrixL().transpose()            imu_factor.h:64
@@ -12,7 +12,7 @@
 //                         (marginalization_factor.cpp:110-297) producing the new prior in information form
 // The solve replaces ceres::Solve(DENSE_SCHUR, DOGLEG) at estimator.cpp:803-818; no wall-clock cap.
 // Everything here is small dense float64 algebra: latency bound for one sequence, HBM bound in batches;
-// B200's FP64 pipe is far from saturated, so no tensor-core path is used (see DESIGN.md).
+// the FP64 pipe is far from saturated, so no tensor-core path is used (see DESIGN.md).
 #include "ba_kernels.h"
 
 #include <algorithm>

@@ -1443,7 +1443,9 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
     } while (0)
     VE_TRY(cudaSetDevice(cfg->device));
     // launch groups: VINSB200_BATCH_GROUPS overrides the default (two groups for batches of 32 members and more)
-    int G = n >= 32 ? 2 : 1;  // measured on B200 with 64 members: 1 group 8.66 k, 2 groups 9.50 k, 4 groups 9.26 k, 8 groups 8.45 k frames/s
+    // measured on an H100 SXM (400 W limit), 64 members, two alternating runs each: 1 group 6.50 / 6.55 k, 2 groups
+    // 6.78 / 5.91 k, 3 groups 6.71 / 6.37 k, 4 groups 6.89 / 6.69 k frames/s, i.e. within the run-to-run spread
+    int G = n >= 32 ? 2 : 1;
     if (const char* env = std::getenv("VINSB200_BATCH_GROUPS")) G = std::atoi(env);
     G = std::max(1, std::min(G, n));
     b->G = G;

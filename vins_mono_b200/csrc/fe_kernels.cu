@@ -1,4 +1,4 @@
-// Front-end image kernels for sm_100a (feature_tracker hot path, SURVEY.md §8 rows a3, a4, a7, a8).
+// Front-end image kernels for sm_90a (feature_tracker hot path, SURVEY.md §8 rows a3, a4, a7, a8).
 //
 // Every kernel reproduces the integer / IEEE-f32 arithmetic of the OpenCV routine the reference calls
 // (feature_tracker/src/feature_tracker.cpp:87-93 CLAHE, :113 calcOpticalFlowPyrLK, :66 circle,
