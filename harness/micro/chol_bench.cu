@@ -11,7 +11,7 @@ __global__ void __launch_bounds__(512) chol_bench_kernel(const double* Ain, int 
     extern __shared__ __align__(16) double dyn[];
     double* Pc = dyn;
     double* Lp = dyn + CHOL_NB * CHOL_PS;
-    __shared__ double rdiag[STEP_MAXD], linv[(STEP_MAXD / CHOL_NB) * 64], y[STEP_MAXD];
+    __shared__ double rdiag[BA_MAX_D], linv[(BA_MAX_D / CHOL_NB) * 64], y[BA_MAX_D];
     __shared__ int flag;
     const int np = n * (n + 1) / 2;
     if (threadIdx.x < 8) chol_clk[threadIdx.x] = 0;

@@ -15,7 +15,6 @@
 
 namespace vb {
 
-constexpr int RED_MAXD = 352;       // 15 (W + 1) + 7 for W <= 22
 constexpr int RED_THREADS = 256;
 
 #define LIN_WARPS 4
@@ -209,7 +208,6 @@ __device__ inline void lin_imu(const BaProblem& p, const BaStates& x, const BaAc
     }
 }
 
-#define PRIOR_MAX_N 160
 
 // dx of the prior's kept blocks (MarginalizationFactor::Evaluate, marginalization_factor.cpp:343-364)
 __device__ __forceinline__ void prior_dx(const BaProblem& p, const BaStates& x, double* dx, int tid, int nthreads) {
@@ -266,7 +264,7 @@ __device__ inline void lin_prior(const BaProblem& p, const BaStates& x, const Ba
 template <bool EX, bool TD>
 __global__ void __launch_bounds__(32 * LIN_WARPS, 3) ba_eval_kernel(const BaSeq* __restrict__ seqs, int initial) {
     __shared__ double sJraw[450], srr[16];
-    __shared__ double sdx[PRIOR_MAX_N], sred[PRIOR_MAX_N];
+    __shared__ double sdx[BA_MAX_PRIOR_N], sred[BA_MAX_PRIOR_N];
     __shared__ BaProblem sp;
     __shared__ int is_last;
     const BaSeq& q = seqs[blockIdx.y];
@@ -532,7 +530,7 @@ constexpr int RED_SLAB = 1024;
 template <bool RELO>
 __global__ void __launch_bounds__(RED_THREADS, 3) ba_reduce_kernel(const BaSeq* __restrict__ seqs, int n_pairs_max) {
     __shared__ BaProblem sp;
-    __shared__ int pinv[RED_MAXD];
+    __shared__ int pinv[BA_MAX_D];
     __shared__ short s_an[RED_SLAB], s_nobs[RED_SLAB];
     __shared__ unsigned char s_rl[RED_SLAB];
     __shared__ int s_s0[RED_SLAB];

@@ -14,6 +14,7 @@
 // Everything here is small dense float64 algebra: latency bound for one sequence, HBM bound in batches;
 // the FP64 pipe is far from saturated, so no tensor-core path is used (see DESIGN.md).
 #include "ba_kernels.h"
+#include "ba_layout.h"
 
 #include <algorithm>
 #include <mutex>
@@ -306,7 +307,7 @@ __device__ double quad_form(const BaProblem& p, const BaAccum& a, const double* 
 // (8 dependent rsqrt + shuffle rounds) off the critical path.  The panel below a diagonal block is solved by one
 // thread per row, trailing tiles are 4x4 register tiles (0.5 shared-memory loads per FMA).  3 barriers per block column.
 #define CHOL_NB 8
-#define CHOL_PS 360  // panel copy stride: STEP_MAXD + 8 rows of slack for partial tiles
+#define CHOL_PS 360  // panel copy stride: BA_MAX_D + 8 rows of slack for partial tiles
 #ifdef CHOL_PROF  // harness/micro/chol_bench.cu: per-phase cycle counters kept in shared memory by thread 0
 __shared__ long long chol_clk[8];
 #define CP_BEGIN() long long cp0_ = clock64()
@@ -646,11 +647,10 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
         : "memory");
 }
 
-#define STEP_MAXD 352
 __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ seqs, int use_smem_chol) {
     extern __shared__ __align__(16) double chol_smem[];  // panel copy (CHOL_NB * CHOL_PS), then the packed factor
     __shared__ double red[32];
-    __shared__ double rdiag[STEP_MAXD], ysm[STEP_MAXD], linv[(STEP_MAXD / CHOL_NB) * 64];
+    __shared__ double rdiag[BA_MAX_D], ysm[BA_MAX_D], linv[(BA_MAX_D / CHOL_NB) * 64];
     __shared__ int flag;
     __shared__ BaProblem sp;
     const BaSeq& q = seqs[blockIdx.x];
@@ -672,10 +672,11 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
     const int lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
     const int cur = st->cur;
     const BaAccum a = p.acc[cur];
-    double* u = p.work;              // N  Cauchy direction (unscaled variables)
-    double* y = p.work + N;          // N  Gauss-Newton solution
-    double* delta = p.work + 2 * N;  // N  step in the original variables
-    double* Lp = use_smem_chol ? chol_smem + CHOL_NB * CHOL_PS : p.work + 4 * (size_t)N;  // packed factor
+    const BaWorkLayout wl = ba_work_layout(D, L);
+    double* u = p.work + wl.u;          // Cauchy direction (unscaled variables)
+    double* y = p.work + wl.y;          // Gauss-Newton solution
+    double* delta = p.work + wl.delta;  // step in the original variables
+    double* Lp = use_smem_chol ? chol_smem + CHOL_NB * CHOL_PS : p.work + wl.Lp;  // packed factor
     const int first = st->first;
     double mu = st->mu;
     bool linear_ok = true;
@@ -683,7 +684,7 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
 #define STAMP(k) do { if (tid == 0) { const long long c1_ = clock64(); st->clk[k] += c1_ - c0; c0 = c1_; } } while (0)
     const int npk0 = D * (D + 1) / 2;
     // cp.async.bulk moves multiples of 16 bytes: an odd count is rounded up, the extra double lands on Lp[npk0] (the first
-    // entry of the right-hand-side row, written after the transfer has completed; Spk is allocated for the largest D)
+    // entry of the right-hand-side row, written after the transfer has completed; Spk has BA_SPK_SLACK behind the largest D)
     const unsigned copy_bytes = (unsigned)(((npk0 + 1) & ~1) * sizeof(double));
     const bool bulk_ok = use_smem_chol != 0;
     bool copy_in_flight = false;
@@ -936,7 +937,7 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
 // same device code as the solve's linearisation, with the extrinsic block always live: it is a parameter of the prior even
 // when the solve keeps it constant), then the dense system is gathered entry by entry in a fixed order (marg_gather_kernel).
 constexpr int MARG_OJ = OJ_FULL, MARG_LW = LW_FULL;
-constexpr int MARG_QMAX = 160 + 16;  // non-landmark columns: m_dense (<= 15) + kept (<= 160)
+constexpr int MARG_QMAX = BA_MARG_MAX_DENSE + 1 + BA_MAX_PRIOR_N;  // non-landmark columns: m_dense + kept, and one spare
 
 // Clears the members' marginalisation systems (Am P x P, bm P).
 __global__ void __launch_bounds__(256) marg_zero_kernel(const BaSeq* __restrict__ seqs) {
@@ -954,7 +955,7 @@ __global__ void __launch_bounds__(256) marg_zero_kernel(const BaSeq* __restrict_
 template <bool TD>
 __global__ void __launch_bounds__(32 * LIN_WARPS) marg_eval_kernel(const BaSeq* __restrict__ seqs) {
     __shared__ double sJraw[450], srr[16];
-    __shared__ double sdx[PRIOR_MAX_N], sred[PRIOR_MAX_N];
+    __shared__ double sdx[BA_MAX_PRIOR_N], sred[BA_MAX_PRIOR_N];
     __shared__ BaProblem sp;
     const BaSeq& q = seqs[blockIdx.y];
     if (!q.active || !q.do_marg) return;
@@ -1107,7 +1108,6 @@ __global__ void __launch_bounds__(128) marg_gather_kernel(const BaSeq* __restric
 }
 
 constexpr int MARG_THREADS = 512;
-constexpr int MARG_MAXN = 160;  // kept prior parameters (6 W + 9 + 6 + 1) supported by the work arrays: WINDOW_SIZE <= 22
 
 // doubles of the scratch area Ev: staged landmark rows (2 x 16 x qp) or the n x md products Y and X
 // (+ a copy of the scaled eigenvectors, n x (n|1), when the reduced system lives in shared memory, i.e. small windows)
@@ -1130,7 +1130,7 @@ __host__ __device__ inline int marg_scratch_doubles(int md, int n, bool w_in_glo
 __global__ void __launch_bounds__(MARG_THREADS) marg_solve_kernel(const BaSeq* __restrict__ seqs, double eps) {
     extern __shared__ __align__(16) double sm[];
     __shared__ double red[32];
-    __shared__ double dval[MARG_MAXN], ework[MARG_MAXN], cs[4 * MARG_MAXN], scal[16];
+    __shared__ double dval[BA_MAX_PRIOR_N], ework[BA_MAX_PRIOR_N], cs[4 * BA_MAX_PRIOR_N], scal[16];
     __shared__ MargPlan smp;
     {
         const BaSeq& q = seqs[blockIdx.x];
@@ -1381,11 +1381,12 @@ __global__ void __launch_bounds__(MARG_THREADS) marg_solve_kernel(const BaSeq* _
             prior_floor<CtaCtx, SE_PER_LANE_MAX>(CtaCtx(), Ap, mp.gout, mp.cout, n, eps, Vv, ldvn, dval, ework, cs, scal, tv, fwork, fev, fstats);
     }
     MSTAMP(3);
-    if (tid == 0 && mp.graw) {  // diagnostics behind the n used entries
-        mp.graw[n] = scal[4];              // A' decomposition: tridiagonalisation cycles
-        mp.graw[n + 1] = (double)fstats[0];  // eigenpairs separated explicitly (-1: full decomposition)
+    if (tid == 0 && mp.graw) {  // the BA_MARG_DIAG diagnostics behind the n used entries
+        double* diag = mp.graw + n;
+        diag[0] = scal[4];              // A' decomposition: tridiagonalisation cycles
+        diag[1] = (double)fstats[0];  // eigenpairs separated explicitly (-1: full decomposition)
         MSTAMP(4);
-        for (int k = 0; k < 5; k++) mp.graw[n + 2 + k] = (double)mclk[k];
+        for (int k = 0; k < BA_MARG_DIAG - 2; k++) diag[2 + k] = (double)mclk[k];
     }
 }
 
@@ -1402,7 +1403,7 @@ size_t marg_solve_smem_bytes(int m_dense, int n, bool w_in_global) {
 // degrees of freedom), written to the member's output block for the host (Ps, Rs, Vs, Bas, Bgs, tic, ric, td, depths)
 // and packed again into x[0], the linearisation point of this frame's marginalisation; the new prior's x0 is taken from it.
 __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs) {
-    __shared__ double sin_[BA_MAX_FRAMES * 16 + 8];
+    __shared__ double sin_[ba_states_layout(BA_MAX_FRAMES, 0).lam];  // pose | sb | ex | td of x[cur] (the states layout)
     __shared__ double rot[9];
     BaSeq& q = seqs[blockIdx.x];
     if (!q.active) return;
@@ -1412,13 +1413,14 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
     const int F = p.dims.W + 1, L = p.dims.L;
     const int cur = q.st.cur;
     const BaStates xs = p.x[cur], xd = p.x[0];
-    for (int i = tid; i < 7 * F; i += nt) sin_[i] = xs.pose[i];
-    for (int i = tid; i < 9 * F; i += nt) sin_[7 * F + i] = xs.sb[i];
-    for (int i = tid; i < 7; i += nt) sin_[16 * F + i] = xs.ex[i];
-    if (tid == 0) sin_[16 * F + 7] = xs.td[0];
+    const BaStates sx = states_view(sin_, F, 0);
+    for (int i = tid; i < 7 * F; i += nt) sx.pose[i] = xs.pose[i];
+    for (int i = tid; i < 9 * F; i += nt) sx.sb[i] = xs.sb[i];
+    for (int i = tid; i < 7; i += nt) sx.ex[i] = xs.ex[i];
+    if (tid == 0) sx.td[0] = xs.td[0];
     __syncthreads();
     if (tid == 0) {
-        const M3d R00 = qR(q_from_param(sin_));
+        const M3d R00 = qR(q_from_param(sx.pose));
         const V3d o0 = mk(fp.origin_ypr[0], fp.origin_ypr[1], fp.origin_ypr[2]);
         const V3d o00 = R2ypr_dev(R00);
         const double y_diff = o0.x - o00.x;
@@ -1436,16 +1438,16 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
         const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&q.st);
         for (int i = tid; i < (int)(sizeof(SolverState) / 8); i += nt) reinterpret_cast<unsigned long long*>(out)[i] = src[i];
     }
-    double* of = out + BA_OUT_ST_DOUBLES;
+    const BaOutLayout ol = ba_out_layout(F, L, p.dims.col_relo >= 0);
     M3d rd;
     for (int k = 0; k < 9; k++) rd.m[k] = rot[k];
     for (int f = tid; f < F; f += nt) {
-        const double* pp = sin_ + 7 * f;
-        const double* sbp = sin_ + 7 * F + 9 * f;
+        const double* pp = sx.pose + 7 * f;
+        const double* sbp = sx.sb + 9 * f;
         const M3d R = mmul(rd, qR(qnormalized(q_from_param(pp))));
-        const V3d P = mv(rd, mk(pp[0] - sin_[0], pp[1] - sin_[1], pp[2] - sin_[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
+        const V3d P = mv(rd, mk(pp[0] - sx.pose[0], pp[1] - sx.pose[1], pp[2] - sx.pose[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
         const V3d V = mv(rd, mk(sbp[0], sbp[1], sbp[2]));
-        double* o = of + 21 * f;
+        double* o = out + ol.frames + BA_OUT_FRAME * f;
         o[0] = P.x; o[1] = P.y; o[2] = P.z;
         for (int k = 0; k < 9; k++) o[3 + k] = R.m[k];
         o[12] = V.x; o[13] = V.y; o[14] = V.z;
@@ -1459,26 +1461,26 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
         for (int k = 0; k < 6; k++) ds[3 + k] = sbp[3 + k];
     }
     if (tid == nt - 1) {
-        const double* xe = sin_ + 16 * F;
+        const double* xe = sx.ex;
         const M3d ric = qR(q_from_param(xe));
-        double* o = of + 21 * F;
+        double* o = out + ol.ex;
         o[0] = xe[0]; o[1] = xe[1]; o[2] = xe[2];
         for (int k = 0; k < 9; k++) o[3 + k] = ric.m[k];
-        o[12] = xe[7];
+        o[12] = sx.td[0];
         const Q4 qq = q_from_R(ric);
         xd.ex[0] = xe[0]; xd.ex[1] = xe[1]; xd.ex[2] = xe[2];
         xd.ex[3] = qq.x; xd.ex[4] = qq.y; xd.ex[5] = qq.z; xd.ex[6] = qq.w;
-        xd.td[0] = xe[7];
+        xd.td[0] = sx.td[0];
     }
     if (tid == nt - 2 && p.dims.col_relo >= 0) {  // relo_r / relo_t of double2vector (estimator.cpp:598-605)
         const double* rp = xs.relo;
         const M3d Rr = mmul(rd, qR(qnormalized(q_from_param(rp))));
-        const V3d Pr = mv(rd, mk(rp[0] - sin_[0], rp[1] - sin_[1], rp[2] - sin_[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
-        double* o = of + 21 * F + 13 + L;
+        const V3d Pr = mv(rd, mk(rp[0] - sx.pose[0], rp[1] - sx.pose[1], rp[2] - sx.pose[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
+        double* o = out + ol.relo;
         for (int k = 0; k < 9; k++) o[k] = Rr.m[k];
         o[9] = Pr.x; o[10] = Pr.y; o[11] = Pr.z;
     }
-    double* od = of + 21 * F + 13;
+    double* od = out + ol.depths;
     for (int l = tid; l < L; l += nt) {  // FeatureManager::setDepth, then getDepthVector
         const double dep = 1.0 / xs.lam[l];
         od[l] = dep;
@@ -1544,8 +1546,6 @@ __global__ void __launch_bounds__(32) debug_imu_kernel(BaDims d, const PreInt* _
 // ------------------------------------------------------------------------------------------------
 // launch wrappers
 namespace vb {
-
-size_t ba_work_doubles(int D, int L) { return 4 * (size_t)(D + L) + (size_t)(D + 1) * (D + 2) / 2; }
 
 namespace {
 

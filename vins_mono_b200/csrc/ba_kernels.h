@@ -30,7 +30,6 @@ void launch_preint_jobs(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* 
 // linearise + decide}; then the device-side double2vector / vector2double (results into the members' output blocks).
 void launch_ba_solve(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* launches, KernelProfile* prof = nullptr);
 void launch_marginalize(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* launches, KernelProfile* prof = nullptr);
-size_t ba_work_doubles(int D, int L);
 // Whether marg_solve_kernel keeps its reduced system in global memory for these sizes on the current device.
 int marg_w_in_global(int m_dense, int n);
 

@@ -7,7 +7,6 @@
 // these in device memory; every kernel takes the array and picks its member with a grid dimension, so one launch
 // per stage serves the whole batch (S = 1 is the single-sequence path, the same code).
 #pragma once
-#include <cuda_runtime.h>
 #include <cstdint>
 
 namespace vb {
@@ -15,6 +14,11 @@ namespace vb {
 constexpr int BA_MAX_OBS_PER_LM = 32;  // lanes of the landmark warp (window size + 1 <= 32)
 constexpr int BA_MAX_FRAMES = 32;
 constexpr int BA_MAX_PRIOR_BLOCKS = 64;
+// Capacity of the single-CTA solvers' work arrays, which fixes WINDOW_SIZE <= 22 (the reference ships 10):
+constexpr int BA_MAX_D = 352;        // reduced (camera-side) system columns: 15 (W + 1) + 6 + 1 at W = 22
+constexpr int BA_MAX_PRIOR_N = 160;  // prior parameters: 6 W + 9 + 6 + 1
+constexpr int BA_MARG_MAX_DENSE = 15;  // marginalised non-landmark columns: a pose and a speed-bias block
+constexpr int BA_MARG_DIAG = 7;        // diagnostics marg_solve_kernel writes behind the n entries of MargPlan::graw
 
 struct PreInt {  // IntegrationBase (integration_base.h:189-209) + cached sqrt_info (imu_factor.h:64)
     double sum_dt;
@@ -57,19 +61,19 @@ struct BaStates {  // one point x: Ceres parameter layouts
 //         Hii = sum Ji^T Ji (21, packed upper) | gi = sum Ji^T r 6 | wi = sum Ji^T Jl 6 | Hll | gl | cost |
 //         [Hie 6x6 | Hee 21 | ge 6 | we 6] [Hit 6 | Het 6 | Htt | gt | wt]
 //   imuJ  per IMU factor k (stride 480): whitened Jacobian 15x30 | whitened residual 15 | cost | valid
-//   gpr   prior gradient g0 + A dx (n), cost of the prior at gpr[BA_PRIOR_COST]
+//   gpr   prior gradient g0 + A dx (n <= BA_MAX_PRIOR_N), cost of the prior at gpr[BA_PRIOR_COST]
 enum : int {
     OJ_JI = 0, OJ_JJ = 12, OJ_R = 24, OJ_JL = 26, OJ_WJ = 28, OJ_BASE = 34, OJ_JEX = 34, OJ_JTD = 46, OJ_FULL = 48,
     LW_HII = 0, LW_GI = 21, LW_WI = 27, LW_HLL = 33, LW_GL = 34, LW_COST = 35, LW_BASE = 36,
     LW_HIE = 36, LW_HEE = 72, LW_GE = 93, LW_WE = 99, LW_HIT = 105, LW_HET = 111, LW_HTT = 117, LW_GT = 118, LW_WT = 119, LW_FULL = 120,
     IMUJ_JW = 0, IMUJ_RW = 450, IMUJ_COST = 465, IMUJ_VALID = 466, IMUJ_STRIDE = 480,
-    BA_PRIOR_COST = 160
+    BA_PRIOR_COST = BA_MAX_PRIOR_N
 };
 struct BaAccum {
     double* obsJ;  // M x oj
     double* lmW;   // L x lw
     double* imuJ;  // W x IMUJ_STRIDE
-    double* gpr;   // BA_PRIOR_COST + 1
+    double* gpr;   // BA_PRIOR_COST + 8: n gradient entries, the prior's cost at gpr[BA_PRIOR_COST], padding
     double* gp;    // D: gradient of the camera-side parameters (written by ba_reduce_kernel)
     double* cost;  // 1: total cost, summed in a fixed order by the last CTA of ba_eval_kernel
 };
@@ -131,7 +135,7 @@ struct BaProblem {
     double* diag;    // D + L trust-region diagonal
     double* grad;    // D + L
     double* gn;      // D + L
-    double* work;    // 4 x (D + L) scratch
+    double* work;    // step scratch and the packed Cholesky factor (ba_work_layout, ba_layout.h)
     SolverState* st; // points at BaSeq::st of the same member
 };
 
@@ -149,7 +153,7 @@ struct MargPlan {  // dense marginalisation system layout: [m_dense | n_lm landm
     double* gout;       // n       new prior g0
     double* cout;       // 1       new prior c0
     double* Araw;       // n x n   Schur complement before the eps floor (tests), may be null
-    double* graw;       // n (+ 7 diagnostics)
+    double* graw;       // n (+ BA_MARG_DIAG diagnostics)
     double* Wglobal;    // q x q scratch (q = m_dense + n) used when the reduced system does not fit shared memory
 };
 
@@ -165,8 +169,7 @@ struct FinishPlan {
     double origin_ypr[3];  // R2ypr(Rs[0]) before the solve (degrees), or of last_R0 after a detected failure
     double origin_P0[3];
     double Rs0[9];         // Rs[0] before the solve (Euler-singularity fallback)
-    double* out;           // member's output block: SolverState | (W+1) x 21 (P, R row-major, V, Ba, Bg) | tic 3 | ric 9 | td | L depths |
-                           // with a relocalisation block: relo_r 9 (row-major) | relo_t 3 (estimator.cpp:598-605)
+    double* out;           // member's output block (ba_out_layout, ba_layout.h); relo_r / relo_t: estimator.cpp:598-605
     int n_kept;            // kept blocks of the new prior (0: nothing is marginalised this frame)
     int kept_type[BA_MAX_PRIOR_BLOCKS], kept_index[BA_MAX_PRIOR_BLOCKS];  // pre-shift identities
     double* x0_out;        // new prior's linearisation point, 9 doubles per kept block

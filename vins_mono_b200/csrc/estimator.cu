@@ -26,6 +26,8 @@
 #include <vector>
 
 #include "ba_kernels.h"
+#include "ba_layout.h"
+#include "cuda_check.h"
 #include "host_math.h"
 #include <array>
 
@@ -206,32 +208,6 @@ struct ve_batch {
 
 namespace {
 
-#define VE_CUDA(call)                                                        \
-    do {                                                                     \
-        cudaError_t e_ = (call);                                             \
-        if (e_ != cudaSuccess) {                                             \
-            e->err = std::string(#call) + ": " + cudaGetErrorString(e_);     \
-            return VE_ERR_CUDA;                                              \
-        }                                                                    \
-    } while (0)
-
-size_t states_doubles(const ve_estimator* e, int L) { return (size_t)(e->W + 1) * 16 + 8 + L + 8; }  // ... | lam L | relo_Pose 7 (+1)
-// per-factor linearisation records of one point (BaAccum): obsJ | lmW | imuJ | gpr | gp | cost, at the widest strides
-size_t acc_doubles(const ve_estimator* e) {
-    return (size_t)e->Mmax * vb::OJ_FULL + (size_t)e->Lmax * vb::LW_FULL + (size_t)e->W * vb::IMUJ_STRIDE + (vb::BA_PRIOR_COST + 8) + e->D + 8;
-}
-size_t align16(size_t bytes) { return (bytes + 15) & ~(size_t)15; }
-
-vb::BaStates states_view(double* p, int F, int L) {
-    vb::BaStates s;
-    s.pose = p;
-    s.sb = p + 7 * F;
-    s.ex = p + 16 * F;
-    s.td = p + 16 * F + 7;
-    s.lam = p + 16 * F + 8;
-    s.relo = s.lam + L;
-    return s;
-}
 bool usable(const ve_estimator* e, FeaturePerId& it) {  // the filter repeated all over feature_manager.cpp
     it.used_num = (int)it.feature_per_frame.size();
     return it.used_num >= 2 && it.start_frame < e->W - 2;
@@ -616,46 +592,45 @@ bool failure_detection(ve_estimator* e) {
     return false;
 }
 
-// vector2double (estimator.cpp:486-528): packs the window into the staging layout pose|sb|ex|td|lam
-void pack_states(ve_estimator* e, double* out) {
+// vector2double (estimator.cpp:486-528): packs the window into a states vector whose view `x` has room for its landmarks
+void pack_states(ve_estimator* e, const vb::BaStates& x) {
     const int F = e->W + 1;
     for (int i = 0; i < F; i++) {
         const Quat q = Quat::FromR(e->Rs[i]);
-        double* p = out + 7 * i;
+        double* p = x.pose + 7 * i;
         p[0] = e->Ps[i].x; p[1] = e->Ps[i].y; p[2] = e->Ps[i].z; p[3] = q.x; p[4] = q.y; p[5] = q.z; p[6] = q.w;
-        double* s = out + 7 * F + 9 * i;
+        double* s = x.sb + 9 * i;
         s[0] = e->Vs[i].x; s[1] = e->Vs[i].y; s[2] = e->Vs[i].z;
         s[3] = e->Bas[i].x; s[4] = e->Bas[i].y; s[5] = e->Bas[i].z;
         s[6] = e->Bgs[i].x; s[7] = e->Bgs[i].y; s[8] = e->Bgs[i].z;
     }
     const Quat q = Quat::FromR(e->ric);
-    double* x = out + 16 * F;
-    x[0] = e->tic.x; x[1] = e->tic.y; x[2] = e->tic.z; x[3] = q.x; x[4] = q.y; x[5] = q.z; x[6] = q.w;
-    out[16 * F + 7] = e->td;
+    x.ex[0] = e->tic.x; x.ex[1] = e->tic.y; x.ex[2] = e->tic.z; x.ex[3] = q.x; x.ex[4] = q.y; x.ex[5] = q.z; x.ex[6] = q.w;
+    x.td[0] = e->td;
     int k = 0;
     for (auto& it : e->feature)
-        if (usable(e, it)) out[16 * F + 8 + k++] = 1. / it.estimated_depth;
-    for (int q7 = 0; q7 < 7; q7++) out[16 * F + 8 + k + q7] = e->relo_Pose[q7];
+        if (usable(e, it)) x.lam[k++] = 1. / it.estimated_depth;
+    for (int q7 = 0; q7 < 7; q7++) x.relo[q7] = e->relo_Pose[q7];
 }
 
 // Results of the device-side double2vector (ba_finish_kernel) -> Estimator members.
 void unpack_results(ve_estimator* e, const double* out) {
     const int F = e->W + 1;
+    const vb::BaOutLayout ol = vb::ba_out_layout(F, e->fr_L, e->fr_relo);
     std::memcpy(&e->last_state, out, sizeof(vb::SolverState));
-    const double* of = out + vb::BA_OUT_ST_DOUBLES;
     for (int i = 0; i < F; i++) {
-        const double* o = of + 21 * i;
+        const double* o = out + ol.frames + vb::BA_OUT_FRAME * i;
         e->Ps[i] = Vec3(o[0], o[1], o[2]);
         std::memcpy(e->Rs[i].m, o + 3, 9 * sizeof(double));
         e->Vs[i] = Vec3(o[12], o[13], o[14]);
         e->Bas[i] = Vec3(o[15], o[16], o[17]);
         e->Bgs[i] = Vec3(o[18], o[19], o[20]);
     }
-    const double* x = of + 21 * F;
+    const double* x = out + ol.ex;
     e->tic = Vec3(x[0], x[1], x[2]);
     std::memcpy(e->ric.m, x + 3, 9 * sizeof(double));
     if (e->cfg.estimate_td) e->td = x[12];
-    const double* od = x + 13;
+    const double* od = out + ol.depths;
     int k = 0;
     for (auto& it : e->feature) {  // FeatureManager::setDepth
         if (!usable(e, it)) continue;
@@ -667,7 +642,7 @@ void unpack_results(ve_estimator* e, const double* out) {
         e->para_Pose[i] = {e->Ps[i].x, e->Ps[i].y, e->Ps[i].z, q.x, q.y, q.z, q.w};
     }
     if (e->fr_relo) {  // drift bookkeeping of double2vector (estimator.cpp:598-617); relo_r / relo_t come from the device
-        const double* ro = od + k;
+        const double* ro = out + ol.relo;
         Mat3 relo_r;
         std::memcpy(relo_r.m, ro, 9 * sizeof(double));
         const Vec3 relo_t(ro[9], ro[10], ro[11]);
@@ -751,7 +726,7 @@ int plan_marginalization(ve_estimator* e, vb::MargPlan& mp, MargHost& mh) {
     if (t_td) { mp.col_td = pos; mh.kept.push_back({3, 0, pos - m, 1}); pos += 1; }
     mp.P = pos;
     mp.n = pos - m;
-    if (mp.n > e->nmax || mp.P > e->nmax + 15 + e->Lmax || mp.m_dense == 0 || (int)mh.kept.size() > vb::BA_MAX_PRIOR_BLOCKS) {
+    if (mp.n > e->nmax || mp.P > (int)vb::ba_marg_layout(e->nmax, e->Lmax).P || mp.m_dense == 0 || (int)mh.kept.size() > vb::BA_MAX_PRIOR_BLOCKS) {
         e->err = "marginalisation system larger than the configured capacity";
         return VE_ERR_CAPACITY;
     }
@@ -786,9 +761,9 @@ int stage_frame(ve_estimator* e, bool solve) {
     if (solve) {
         for (int f = 0; f <= W; f++) flush_frame(e, f);
         q.sqrt_mask = refresh_sqrt_mask(e);
-        // the solver's column tables hold 352 entries (W = 22 with extrinsic and td): a relocalisation block that would not fit is
-        // left out (only possible at the largest window with both optional blocks live)
-        const bool relo = e->relocalization_info && 15 * F + 6 * (e->cfg.estimate_extrinsic ? 1 : 0) + (e->cfg.estimate_td ? 1 : 0) + 6 <= 352;
+        // the solver's column tables hold BA_MAX_D entries (W = 22 with extrinsic and td): a relocalisation block that would not
+        // fit is left out (only possible at the largest window with both optional blocks live)
+        const bool relo = e->relocalization_info && 15 * F + 6 * (e->cfg.estimate_extrinsic ? 1 : 0) + (e->cfg.estimate_td ? 1 : 0) + 6 <= vb::BA_MAX_D;
         const size_t n_match = e->match_points.size() / 3;
         size_t retrive_feature_index = 0;
         int n_relo = 0;
@@ -825,37 +800,23 @@ int stage_frame(ve_estimator* e, bool solve) {
     const size_t n_jobs = e->jobs.size(), n_rec = e->job_samples.size() / 7;
     if (!solve && n_jobs == 0) return VE_OK;
     const size_t n_lm = mh.lms.size();
-    // layout of the input block (byte offsets, every array 16-byte aligned)
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += align16(bytes);
-        return o;
-    };
-    const size_t o_jobs = take(n_jobs * sizeof(vb::PreintJob)), o_samples = take(n_rec * 7 * sizeof(double));
-    size_t o_int = 0, o_dbl = 0, o_states = 0, o_marg = 0;
-    if (solve) {
-        o_int = take(sizeof(int) * ((size_t)3 * L + 1 + M + W));
-        o_dbl = take(sizeof(double) * (6 * (size_t)L + 6 * (size_t)M));
-        o_states = take(sizeof(double) * states_doubles(e, L));
-        o_marg = take(sizeof(int) * 2 * n_lm);
-    }
+    const vb::BaInLayout il = vb::ba_in_layout(W, n_jobs, n_rec, L, M, n_lm, solve);
     ve_batch::Group& grp = b->groups[e->member / b->members_per_group];
-    const size_t rel = grp.in_used.fetch_add(off);
+    const size_t rel = grp.in_used.fetch_add(il.total);
     const size_t base = grp.in_base + rel;
-    if (rel + off > grp.in_cap) {
+    if (rel + il.total > grp.in_cap) {
         e->err = "batch input arena exhausted";
         return VE_ERR_CAPACITY;
     }
-    unsigned char* hb = b->h_in + base;
-    unsigned char* db = b->d_in + base;
-    e->h2d_bytes = off + sizeof(vb::BaSeq);
+    // the block's arrays in the pinned arena (filled here) and in its device copy (what the kernels read)
+    const vb::BaInPtrs hin = vb::ba_in_bind(b->h_in + base, il), din = vb::ba_in_bind(b->d_in + base, il);
+    e->h2d_bytes = il.total + sizeof(vb::BaSeq);
     // pre-integration jobs
-    if (n_jobs) std::memcpy(hb + o_jobs, e->jobs.data(), n_jobs * sizeof(vb::PreintJob));
-    if (n_rec) std::memcpy(hb + o_samples, e->job_samples.data(), n_rec * 7 * sizeof(double));
+    if (n_jobs) std::memcpy(hin.jobs, e->jobs.data(), n_jobs * sizeof(vb::PreintJob));
+    if (n_rec) std::memcpy(hin.samples, e->job_samples.data(), n_rec * 7 * sizeof(double));
     q.n_jobs = (int)n_jobs;
-    q.jobs = reinterpret_cast<const vb::PreintJob*>(db + o_jobs);
-    q.samples = reinterpret_cast<const double*>(db + o_samples);
+    q.jobs = din.jobs;
+    q.samples = din.samples;
     q.noise[0] = e->cfg.acc_n; q.noise[1] = e->cfg.gyr_n; q.noise[2] = e->cfg.acc_w; q.noise[3] = e->cfg.gyr_w;
     q.p.preint = e->d_preint.p;
     e->jobs.clear();
@@ -863,19 +824,9 @@ int stage_frame(ve_estimator* e, bool solve) {
     if (!solve) return VE_OK;
 
     // ---- observation table grouped by landmark (Estimator::optimization's problem assembly, estimator.cpp:670-801)
-    int* lm_anchor = reinterpret_cast<int*>(hb + o_int);
-    int* lm_start = lm_anchor + L;
-    int* ob_frame = lm_start + L + 1;
-    int* imu_slot = ob_frame + M;
-    int* lm_relo = imu_slot + W;
-    double* lm_pts = reinterpret_cast<double*>(hb + o_dbl);
-    double* lm_vel = lm_pts + 2 * L;
-    double* lm_td = lm_vel + 2 * L;
-    double* lm_row = lm_td + L;
-    double* ob_pts = lm_row + L;
-    double* ob_vel = ob_pts + 2 * M;
-    double* ob_td = ob_vel + 2 * M;
-    double* ob_row = ob_td + M;
+    int *lm_anchor = hin.lm_anchor, *lm_start = hin.lm_start, *ob_frame = hin.ob_frame, *imu_slot = hin.imu_slot, *lm_relo = hin.lm_relo;
+    double *lm_pts = hin.lm_pts, *lm_vel = hin.lm_vel, *lm_td = hin.lm_td, *lm_row = hin.lm_row;
+    double *ob_pts = hin.ob_pts, *ob_vel = hin.ob_vel, *ob_td = hin.ob_td, *ob_row = hin.ob_row;
     int l = 0, m = 0;
     for (auto& it : e->feature) {
         if (!usable(e, it)) continue;
@@ -910,8 +861,7 @@ int stage_frame(ve_estimator* e, bool solve) {
     }
     lm_start[L] = M;
     for (int k = 0; k < W; k++) imu_slot[k] = (e->sum_dt[k + 1] > 10.0 || !e->slot_valid[k + 1]) ? -1 : e->slot_of[k + 1];
-    double* h_states = reinterpret_cast<double*>(hb + o_states);
-    pack_states(e, h_states);
+    pack_states(e, vb::states_view(hin.states, F, L));
 
     vb::BaProblem& p = q.p;
     vb::BaDims& d = p.dims;
@@ -933,41 +883,35 @@ int stage_frame(ve_estimator* e, bool solve) {
     d.tr_over_row = e->cfg.tr / e->cfg.row;
     d.half_row = e->cfg.row / 2;
     d.G[0] = 0; d.G[1] = 0; d.G[2] = e->cfg.g_norm;
-    p.x[0] = states_view(reinterpret_cast<double*>(db + o_states), F, L);
-    p.x[1] = states_view(e->d_states1.p, F, L);
+    p.x[0] = vb::states_view(din.states, F, L);
+    p.x[1] = vb::states_view(e->d_states1.p, F, L);
     const bool wide = d.est_ex || d.est_td;
     d.oj = wide ? vb::OJ_FULL : vb::OJ_BASE;
     d.lw = wide ? vb::LW_FULL : vb::LW_BASE;
+    const vb::BaAccLayout al = vb::ba_acc_layout(W, e->Lmax, e->Mmax, e->D);
     for (int k = 0; k < 2; k++) {  // sized for the widest records; the kernels index with dims.oj / dims.lw
         double* a = e->d_acc[k].p;
-        p.acc[k].obsJ = a;
-        p.acc[k].lmW = a + (size_t)e->Mmax * vb::OJ_FULL;
-        p.acc[k].imuJ = p.acc[k].lmW + (size_t)e->Lmax * vb::LW_FULL;
-        p.acc[k].gpr = p.acc[k].imuJ + (size_t)e->W * vb::IMUJ_STRIDE;
-        p.acc[k].gp = p.acc[k].gpr + vb::BA_PRIOR_COST + 8;
-        p.acc[k].cost = p.acc[k].gp + e->D;
+        p.acc[k] = vb::BaAccum{a + al.obsJ, a + al.lmW, a + al.imuJ, a + al.gpr, a + al.gp, a + al.cost};
     }
-    const int* di = reinterpret_cast<const int*>(db + o_int);
-    p.lm_anchor = di;
-    p.lm_start = di + L;
-    p.ob_frame = di + 2 * L + 1;
-    p.imu_slot = p.ob_frame + M;
-    p.lm_relo = p.imu_slot + W;
-    const double* dobs = reinterpret_cast<const double*>(db + o_dbl);
-    p.lm_pts = dobs;
-    p.lm_vel = dobs + 2 * L;
-    p.lm_td = dobs + 4 * L;
-    p.lm_row = dobs + 5 * L;
-    p.ob_pts = dobs + 6 * L;
-    p.ob_vel = p.ob_pts + 2 * M;
-    p.ob_td = p.ob_vel + 2 * M;
-    p.ob_row = p.ob_td + M;
+    p.lm_anchor = din.lm_anchor;
+    p.lm_start = din.lm_start;
+    p.ob_frame = din.ob_frame;
+    p.imu_slot = din.imu_slot;
+    p.lm_relo = din.lm_relo;
+    p.lm_pts = din.lm_pts;
+    p.lm_vel = din.lm_vel;
+    p.lm_td = din.lm_td;
+    p.lm_row = din.lm_row;
+    p.ob_pts = din.ob_pts;
+    p.ob_vel = din.ob_vel;
+    p.ob_td = din.ob_td;
+    p.ob_row = din.ob_row;
     // current prior
     vb::BaPrior& pr = p.prior;
     pr = vb::BaPrior{};
     vb::BaSeq* dq = b->d_seq + e->member;
+    const vb::BaPriorLayout pl = vb::ba_prior_layout(e->nmax);
     if (e->has_prior) {
-        const int nm = e->nmax;
         pr.n = e->prior_n;
         pr.nblocks = (int)e->prior_blocks.size();
         for (int k = 0; k < pr.nblocks; k++) {
@@ -978,20 +922,21 @@ int stage_frame(ve_estimator* e, bool solve) {
         pr.type = dq->prior_type;  // addresses inside the device copy of this descriptor
         pr.index = dq->prior_index;
         pr.off = dq->prior_off;
-        pr.A = e->d_prior[e->prior_buf].p;
-        pr.g0 = pr.A + (size_t)nm * nm;
-        pr.c0 = pr.g0 + nm;
-        pr.x0 = pr.c0 + 1;
+        const double* a = e->d_prior[e->prior_buf].p;
+        pr.A = a + pl.A;
+        pr.g0 = a + pl.g0;
+        pr.c0 = a + pl.c0;
+        pr.x0 = a + pl.x0;
     }
     p.S = e->d_S.p;
     p.Spk = e->d_Spk.p;
     p.Hfull = e->d_Hfull.p;
     p.gred = e->d_gred.p;
-    const size_t N = (size_t)e->D + e->Lmax;
-    p.scale = e->d_vec.p;
-    p.diag = p.scale + N;
-    p.grad = p.diag + N;
-    p.gn = p.grad + N;
+    const vb::BaVecLayout vl = vb::ba_vec_layout(e->D, e->Lmax);
+    p.scale = e->d_vec.p + vl.scale;
+    p.diag = e->d_vec.p + vl.diag;
+    p.grad = e->d_vec.p + vl.grad;
+    p.gn = e->d_vec.p + vl.gn;
     p.work = e->d_work.p;
     p.st = &dq->st;
     vb::SolverState& st = q.st;
@@ -1012,8 +957,8 @@ int stage_frame(ve_estimator* e, bool solve) {
     fp.origin_ypr[0] = origin_R0.x; fp.origin_ypr[1] = origin_R0.y; fp.origin_ypr[2] = origin_R0.z;
     fp.origin_P0[0] = origin_P0.x; fp.origin_P0[1] = origin_P0.y; fp.origin_P0[2] = origin_P0.z;
     std::memcpy(fp.Rs0, e->Rs[0].m, sizeof(fp.Rs0));
-    const size_t out_doubles = vb::BA_OUT_ST_DOUBLES + 21 * (size_t)F + 13 + L + (e->fr_relo ? 12 : 0);
-    const size_t orel = grp.out_used.fetch_add((out_doubles + 1) & ~(size_t)1);
+    const size_t out_doubles = vb::ba_out_layout(F, L, e->fr_relo).total;
+    const size_t orel = grp.out_used.fetch_add(vb::ba_out_reserve(F, L, e->fr_relo));
     const size_t obase = grp.out_base + orel;
     if (orel + out_doubles > grp.out_cap) {
         e->err = "batch output arena exhausted";
@@ -1026,30 +971,29 @@ int stage_frame(ve_estimator* e, bool solve) {
     fp.x0_out = nullptr;
     // ---- marginalisation
     if (mh.run) {
-        int* h_lms = reinterpret_cast<int*>(hb + o_marg);
         for (size_t k = 0; k < n_lm; k++) {
-            h_lms[k] = mh.lms[k];
-            h_lms[n_lm + k] = mh.col_lm[k];
+            hin.marg_lms[k] = mh.lms[k];
+            hin.marg_col_lm[k] = mh.col_lm[k];
         }
-        mp.lms = reinterpret_cast<const int*>(db + o_marg);
-        mp.col_lm = mp.lms + n_lm;
-        const size_t Pm = (size_t)e->nmax + 15 + e->Lmax;
-        mp.Am = e->d_marg.p;
-        mp.bm = mp.Am + Pm * Pm;
-        mp.Araw = mp.bm + Pm;
-        mp.graw = mp.Araw + (size_t)e->nmax * e->nmax;
-        mp.Wglobal = mp.graw + e->nmax + 8;  // (nmax + 15)^2 doubles
+        mp.lms = din.marg_lms;
+        mp.col_lm = din.marg_col_lm;
+        const vb::BaMargLayout ml = vb::ba_marg_layout(e->nmax, e->Lmax);
+        mp.Am = e->d_marg.p + ml.Am;
+        mp.bm = e->d_marg.p + ml.bm;
+        mp.Araw = e->d_marg.p + ml.Araw;
+        mp.graw = e->d_marg.p + ml.graw;
+        mp.Wglobal = e->d_marg.p + ml.Wglobal;
         mp.w_in_global = b->w_in_global;  // fixed at batch creation
         const int nb = e->prior_buf ^ 1;
-        mp.Aout = e->d_prior[nb].p;  // written with leading dimension n (dense n x n at the front of the buffer)
-        mp.gout = mp.Aout + (size_t)e->nmax * e->nmax;
-        mp.cout = mp.gout + e->nmax;
+        mp.Aout = e->d_prior[nb].p + pl.A;  // written with leading dimension n (dense n x n at the front of the buffer)
+        mp.gout = e->d_prior[nb].p + pl.g0;
+        mp.cout = e->d_prior[nb].p + pl.c0;
         fp.n_kept = (int)mh.kept.size();
         for (int k = 0; k < fp.n_kept; k++) {
             fp.kept_type[k] = mh.kept[k].type;
             fp.kept_index[k] = mh.kept[k].index;
         }
-        fp.x0_out = mp.cout + 1;
+        fp.x0_out = e->d_prior[nb].p + pl.x0;
         q.mp = mp;
         q.do_marg = 1;
         e->fr_marg = true;
@@ -1238,18 +1182,9 @@ struct FrameMsg {
     double stamp;
 };
 
-#define VB_CUDA(call)                                                        \
-    do {                                                                     \
-        cudaError_t e_ = (call);                                             \
-        if (e_ != cudaSuccess) {                                             \
-            b->err = std::string(#call) + ": " + cudaGetErrorString(e_);     \
-            return VE_ERR_CUDA;                                              \
-        }                                                                    \
-    } while (0)
-
 // One frame of the batch: members with a message take part, the others idle.
 int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
-    VB_CUDA(cudaSetDevice(b->cfg.device));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaSetDevice(b->cfg.device));
     const int S = b->S;
     static const bool trace = std::getenv("VINSB200_TRACE") != nullptr;
     const auto t0 = std::chrono::steady_clock::now();
@@ -1309,30 +1244,30 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
             for (int k = grp.first; k < grp.first + grp.count; k++) b->h_seq[k].mp.w_in_global = sh.w_in_global;
         }
         vb::BaSeq* dq = b->d_seq + grp.first;
-        VB_CUDA(cudaMemcpyAsync(dq, b->h_seq + grp.first, sizeof(vb::BaSeq) * grp.count, cudaMemcpyHostToDevice, grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaMemcpyAsync(dq, b->h_seq + grp.first, sizeof(vb::BaSeq) * grp.count, cudaMemcpyHostToDevice, grp.stream));
         const size_t in_bytes = std::min(grp.in_used.load(), grp.in_cap);
-        if (in_bytes) VB_CUDA(cudaMemcpyAsync(b->d_in + grp.in_base, b->h_in + grp.in_base, in_bytes, cudaMemcpyHostToDevice, grp.stream));
-        VB_CUDA(cudaEventRecord(grp.ev[0], grp.stream));
+        if (in_bytes) VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaMemcpyAsync(b->d_in + grp.in_base, b->h_in + grp.in_base, in_bytes, cudaMemcpyHostToDevice, grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[0], grp.stream));
         vb::launch_preint_jobs(dq, sh, grp.stream, &b->last_launches, &b->prof);
-        VB_CUDA(cudaEventRecord(grp.ev[1], grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[1], grp.stream));
         vb::launch_ba_solve(dq, sh, grp.stream, &b->last_launches, &b->prof);
-        VB_CUDA(cudaEventRecord(grp.ev[2], grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[2], grp.stream));
         if (sh.any_active) {  // results travel on the copy stream while the marginalisation already runs
-            VB_CUDA(cudaStreamWaitEvent(grp.copy_stream, grp.ev[2], 0));
+            VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaStreamWaitEvent(grp.copy_stream, grp.ev[2], 0));
             const size_t out_doubles = std::min(grp.out_used.load(), grp.out_cap);
-            VB_CUDA(cudaMemcpyAsync(b->h_out + grp.out_base, b->d_out + grp.out_base, sizeof(double) * out_doubles, cudaMemcpyDeviceToHost,
+            VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaMemcpyAsync(b->h_out + grp.out_base, b->d_out + grp.out_base, sizeof(double) * out_doubles, cudaMemcpyDeviceToHost,
                                     grp.copy_stream));
-            VB_CUDA(cudaEventRecord(grp.ev[4], grp.copy_stream));
+            VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[4], grp.copy_stream));
             grp.waits_results = true;
         } else {
             // jobs only: the input arena must not be rewritten before the copy has been consumed
-            VB_CUDA(cudaEventRecord(grp.ev[4], grp.stream));
+            VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[4], grp.stream));
             grp.waits_results = true;
         }
-        VB_CUDA(cudaEventRecord(grp.ev[5], grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[5], grp.stream));
         vb::launch_marginalize(dq, sh, grp.stream, &b->last_launches, &b->prof);
-        VB_CUDA(cudaEventRecord(grp.ev[3], grp.stream));
-        VB_CUDA(cudaGetLastError());
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventRecord(grp.ev[3], grp.stream));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaGetLastError());
         grp.has_marg = sh.any_marg != 0;
     }
     const double t_launch = since(t1);
@@ -1340,7 +1275,7 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
     for (int g = 0; g < b->G; g++) {
         ve_batch::Group& grp = b->groups[g];
         if (!grp.waits_results) continue;
-        VB_CUDA(cudaEventSynchronize(grp.ev[4]));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaEventSynchronize(grp.ev[4]));
         if (g == 0) {
             float t = 0;
             if (cudaEventElapsedTime(&t, grp.ev[0], grp.ev[1]) == cudaSuccess) b->last_ms[0] = t;
@@ -1376,10 +1311,9 @@ int config_valid(const ve_config* cfg) {
     if (cfg->window_size < 3 || cfg->window_size + 1 > vb::BA_MAX_FRAMES || cfg->window_size + 1 > vb::BA_MAX_OBS_PER_LM ||
         cfg->max_features < 8 || cfg->num_iterations < 1 || cfg->estimate_extrinsic > 2 || cfg->estimate_extrinsic < 0)
         return 0;
-    // work arrays of the single-CTA solvers: prior of 6 W + 9 + 6 + 1 <= 160 parameters, reduced system of
-    // 15 (W + 1) + 7 <= 352 columns, i.e. WINDOW_SIZE <= 22 (the reference ships 10; above 13 the reduced systems
-    // move from shared to global memory)
-    if (6 * cfg->window_size + 16 > 160 || 15 * (cfg->window_size + 1) + 7 > 352) return 0;
+    // work arrays of the single-CTA solvers: prior of 6 W + 9 + 6 + 1 parameters, reduced system of 15 (W + 1) + 7
+    // columns (above W = 13 the reduced systems move from shared to global memory)
+    if (6 * cfg->window_size + 16 > vb::BA_MAX_PRIOR_N || 15 * (cfg->window_size + 1) + 7 > vb::BA_MAX_D) return 0;
     return 1;
 }
 
@@ -1404,15 +1338,15 @@ ve_estimator* create_member(ve_batch* b, int k) {
     e->nmax = 6 * F + 9 * 2 + 6 + 1;
     clear_state(e);
     set_parameter(e);
-    const size_t Pm = (size_t)e->nmax + 15 + e->Lmax;
-    bool ok = e->d_preint.alloc(F) == cudaSuccess && e->d_states1.alloc(states_doubles(e, e->Lmax)) == cudaSuccess;
+    bool ok = e->d_preint.alloc(F) == cudaSuccess && e->d_states1.alloc(vb::ba_states_layout(F, e->Lmax).total) == cudaSuccess;
     for (int k2 = 0; k2 < 2 && ok; k2++)
-        ok = e->d_acc[k2].alloc(acc_doubles(e)) == cudaSuccess &&
-             e->d_prior[k2].alloc((size_t)e->nmax * e->nmax + e->nmax + 1 + 9 * vb::BA_MAX_PRIOR_BLOCKS) == cudaSuccess;
-    ok = ok && e->d_S.alloc((size_t)e->D * e->D) == cudaSuccess && e->d_Spk.alloc((size_t)e->D * (e->D + 1) / 2 + 2)  /* + slack: ba_step's bulk copy rounds an odd count up by one double */ == cudaSuccess &&
+        ok = e->d_acc[k2].alloc(vb::ba_acc_layout(W, e->Lmax, e->Mmax, e->D).total) == cudaSuccess &&
+             e->d_prior[k2].alloc(vb::ba_prior_layout(e->nmax).total) == cudaSuccess;
+    ok = ok && e->d_S.alloc((size_t)e->D * e->D) == cudaSuccess && e->d_Spk.alloc(vb::ba_spk_doubles(e->D)) == cudaSuccess &&
          e->d_Hfull.alloc((size_t)e->D * e->D) == cudaSuccess && e->d_gred.alloc(e->D) == cudaSuccess &&
-         e->d_vec.alloc(4 * ((size_t)e->D + e->Lmax)) == cudaSuccess && e->d_work.alloc(vb::ba_work_doubles(e->D, e->Lmax)) == cudaSuccess &&
-         e->d_marg.alloc(Pm * Pm + Pm + (size_t)e->nmax * e->nmax + e->nmax + 8 + ((size_t)e->nmax + 15) * (e->nmax + 15)) == cudaSuccess;
+         e->d_vec.alloc(vb::ba_vec_layout(e->D, e->Lmax).total) == cudaSuccess &&
+         e->d_work.alloc(vb::ba_work_layout(e->D, e->Lmax).total) == cudaSuccess &&
+         e->d_marg.alloc(vb::ba_marg_layout(e->nmax, e->Lmax).total) == cudaSuccess;
     if (!ok) {
         destroy_member(e);
         return nullptr;
@@ -1437,11 +1371,7 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
         ve_batch_destroy(b);
         return code;
     };
-#define VE_TRY(call)                                          \
-    do {                                                      \
-        if ((call) != cudaSuccess) return fail(VE_ERR_CUDA);  \
-    } while (0)
-    VE_TRY(cudaSetDevice(cfg->device));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaSetDevice(cfg->device));
     // launch groups: VINSB200_BATCH_GROUPS overrides the default (two groups for batches of 32 members and more)
     // measured on an H100 SXM (400 W limit), 64 members, two alternating runs each: 1 group 6.50 / 6.55 k, 2 groups
     // 6.78 / 5.91 k, 3 groups 6.71 / 6.37 k, 4 groups 6.89 / 6.69 k frames/s, i.e. within the run-to-run spread
@@ -1456,9 +1386,9 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
         ve_batch::Group& grp = b->groups[g];
         grp.first = g * b->members_per_group;
         grp.count = std::min(b->members_per_group, n - grp.first);
-        VE_TRY(cudaStreamCreateWithFlags(&grp.stream, cudaStreamNonBlocking));
-        VE_TRY(cudaStreamCreateWithFlags(&grp.copy_stream, cudaStreamNonBlocking));
-        for (auto& ev : grp.ev) VE_TRY(cudaEventCreate(&ev));
+        VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaStreamCreateWithFlags(&grp.stream, cudaStreamNonBlocking));
+        VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaStreamCreateWithFlags(&grp.copy_stream, cudaStreamNonBlocking));
+        for (auto& ev : grp.ev) VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaEventCreate(&ev));
     }
     for (int k = 0; k < n; k++) {
         ve_estimator* e = create_member(b, k);
@@ -1467,11 +1397,7 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
     }
     const ve_estimator* e0 = b->members[0];
     const int W = cfg->window_size, F = W + 1;
-    // input block of one member at full capacity: jobs + samples + tables + states + marginalisation lists
-    const size_t per_in = align16(sizeof(vb::PreintJob) * 4 * F) + align16(sizeof(double) * 7 * 4096) +
-                          align16(sizeof(int) * ((size_t)3 * e0->Lmax + 1 + e0->Mmax + W)) +
-                          align16(sizeof(double) * (6 * (size_t)e0->Lmax + 6 * (size_t)e0->Mmax)) +
-                          align16(sizeof(double) * states_doubles(e0, e0->Lmax)) + align16(sizeof(int) * 2 * (size_t)e0->Lmax);
+    const size_t per_in = vb::ba_in_layout_max(W, e0->Lmax, e0->Mmax).total;  // one member's input block at full capacity
     // a batch rarely has every member at capacity: size the arenas for the full capacity of 8 members or a quarter of
     // the batch, whichever is larger (exhaustion is reported as VE_ERR_CAPACITY, never overrun)
     // per group: full capacity of 4 members or a quarter of the group, whichever is larger, plus a typical share for the rest
@@ -1483,20 +1409,17 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
         grp.in_cap = per_in * at_cap;
         in_total += grp.in_cap;
         grp.out_base = out_total;
-        grp.out_cap = ((size_t)vb::BA_OUT_ST_DOUBLES + 21 * F + 13 + e0->Lmax + 13) * at_cap +
-                      ((size_t)vb::BA_OUT_ST_DOUBLES + 21 * F + 13 + 256 + 12) * (size_t)grp.count;
-        grp.out_cap = (grp.out_cap + 1) & ~(size_t)1;
+        grp.out_cap = vb::ba_out_reserve(F, e0->Lmax, true) * at_cap + vb::ba_out_reserve(F, 256, true) * (size_t)grp.count;
         out_total += grp.out_cap;
     }
-    VE_TRY(cudaMalloc(&b->d_seq, sizeof(vb::BaSeq) * n));
-    VE_TRY(cudaHostAlloc(&b->h_seq, sizeof(vb::BaSeq) * n, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_seq, sizeof(vb::BaSeq) * n));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_seq, sizeof(vb::BaSeq) * n, cudaHostAllocDefault));
     std::memset(b->h_seq, 0, sizeof(vb::BaSeq) * n);
-    VE_TRY(cudaMalloc(&b->d_in, in_total));
-    VE_TRY(cudaHostAlloc(&b->h_in, in_total, cudaHostAllocDefault));
-    VE_TRY(cudaMalloc(&b->d_out, sizeof(double) * out_total));
-    VE_TRY(cudaHostAlloc(&b->h_out, sizeof(double) * out_total, cudaHostAllocDefault));
-#undef VE_TRY
-    b->w_in_global = vb::marg_w_in_global(15, e0->nmax);
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_in, in_total));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_in, in_total, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_out, sizeof(double) * out_total));
+    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_out, sizeof(double) * out_total, cudaHostAllocDefault));
+    b->w_in_global = vb::marg_w_in_global(vb::BA_MARG_MAX_DENSE, e0->nmax);
     b->pool = new vb::HostPool(vb::HostPool::default_workers(n));
     *out = b;
     return VE_OK;
@@ -1577,8 +1500,8 @@ int ve_batch_kernel_times(const ve_batch* b, double* ms8, int* count8) {
 
 int ve_batch_sync(ve_batch* b) {
     if (!b) return VE_ERR_INVALID;
-    VB_CUDA(cudaSetDevice(b->cfg.device));
-    for (int g = 0; g < b->G; g++) VB_CUDA(cudaStreamSynchronize(b->groups[g].stream));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaSetDevice(b->cfg.device));
+    for (int g = 0; g < b->G; g++) VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaStreamSynchronize(b->groups[g].stream));
     return VE_OK;
 }
 
@@ -1797,10 +1720,10 @@ int ve_get_prior(const ve_estimator* ce, int cap, double* A, double* b, int* nbl
     if (n > cap) return -n;
     // the marginalisation that produced the prior may still be running: wait for the batch stream, then read the
     // un-floored Schur complement straight from device memory
-    VE_CUDA(cudaSetDevice(e->cfg.device));
-    VE_CUDA(cudaStreamSynchronize(e->batch->groups[e->member / e->batch->members_per_group].stream));
-    VE_CUDA(cudaMemcpy(A, e->marg_Araw, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
-    VE_CUDA(cudaMemcpy(b, e->marg_graw, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaSetDevice(e->cfg.device));
+    VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaStreamSynchronize(e->batch->groups[e->member / e->batch->members_per_group].stream));
+    VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaMemcpy(A, e->marg_Araw, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
+    VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaMemcpy(b, e->marg_graw, sizeof(double) * n, cudaMemcpyDeviceToHost));
     if (nblocks) *nblocks = (int)e->prior_blocks.size();
     if (blocks4)
         for (size_t k = 0; k < e->prior_blocks.size(); k++) {
@@ -1830,11 +1753,11 @@ int ve_solver_debug(const ve_estimator* ce, double* out18) {
     out18[1] = e->last_state.mu;
     out18[2] = e->last_state.radius;
     for (int k = 0; k < 8; k++) out18[3 + k] = (double)e->last_state.clk[k];
-    double sweeps[7] = {0, 0, 0, 0, 0, 0, 0};
+    double sweeps[vb::BA_MARG_DIAG] = {};  // marg_solve_kernel's diagnostics behind the prior's n entries of graw
     if (e->has_prior && e->marg_graw) {
-        VE_CUDA(cudaSetDevice(e->cfg.device));
-        VE_CUDA(cudaStreamSynchronize(e->batch->groups[e->member / e->batch->members_per_group].stream));
-        VE_CUDA(cudaMemcpy(sweeps, e->marg_graw + e->marg_n, sizeof(sweeps), cudaMemcpyDeviceToHost));
+        VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaSetDevice(e->cfg.device));
+        VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaStreamSynchronize(e->batch->groups[e->member / e->batch->members_per_group].stream));
+        VB_CUDA_CHECK(e, VE_ERR_CUDA, cudaMemcpy(sweeps, e->marg_graw + e->marg_n, sizeof(sweeps), cudaMemcpyDeviceToHost));
     }
     out18[11] = sweeps[0];
     out18[12] = sweeps[1];
@@ -1896,9 +1819,10 @@ int ve_debug_imu_factor(const double* noise4, double g_norm, const double* ba, c
         }
     }
     unsigned char* d = nullptr;
-    const size_t o_seq = 0, o_jobs = align16(sizeof(vb::BaSeq)), o_rec = o_jobs + align16(sizeof(jobs)),
-                 o_pre = o_rec + align16(rec.size() * sizeof(double)), o_prm = o_pre + align16(sizeof(vb::PreInt)),
-                 o_out = o_prm + align16(32 * sizeof(double)), total = o_out + align16(465 * sizeof(double));
+    using vb::ba_align16;
+    const size_t o_seq = 0, o_jobs = ba_align16(sizeof(vb::BaSeq)), o_rec = o_jobs + ba_align16(sizeof(jobs)),
+                 o_pre = o_rec + ba_align16(rec.size() * sizeof(double)), o_prm = o_pre + ba_align16(sizeof(vb::PreInt)),
+                 o_out = o_prm + ba_align16(32 * sizeof(double)), total = o_out + ba_align16(465 * sizeof(double));
     if (cudaMalloc(&d, total) != cudaSuccess) return VE_ERR_CUDA;
     q.n_jobs = 2;
     q.sqrt_mask = 1u;

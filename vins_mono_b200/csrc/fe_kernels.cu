@@ -459,8 +459,8 @@ __global__ void __launch_bounds__(256) mask_init_kernel(const FeSeq* __restrict_
     for (size_t i = i0; i < n16; i += stride) m16[i] = s16 ? s16[i] : make_uint4(~0u, ~0u, ~0u, ~0u);
     for (size_t i = n16 * 16 + i0; i < total; i += stride) q.mask[i] = q.mask_init ? q.mask_init[i] : (uint8_t)255;
     if (i0 == 0) {
-        q.count[0] = 0;
-        q.count[1] = 0;
+        q.count[FE_COUNT_CANDIDATES] = 0;
+        q.count[FE_COUNT_SELECTED] = 0;
         *q.maxv = 0u;
     }
 }
@@ -589,7 +589,7 @@ __global__ void __launch_bounds__(256) gftt_candidates_kernel(const FeSeq* __res
     const uint8_t* __restrict__ mask = q.use_mask ? q.mask : nullptr;
     const unsigned* __restrict__ max_sortable = q.maxv;
     unsigned long long* __restrict__ keys = q.keys;
-    int* __restrict__ count = q.count;
+    int* __restrict__ count = q.count + FE_COUNT_CANDIDATES;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x < 1 || y < 1 || x >= cols - 1 || y >= rows - 1) return;
@@ -621,7 +621,7 @@ __global__ void __launch_bounds__(1024) sort_keys_desc_kernel(const FeSeq* __res
     const FeSeq& q = seqs[blockIdx.x];
     if (!q.detect) return;
     unsigned long long* __restrict__ keys = q.keys;
-    const int* __restrict__ count = q.count;
+    const int* __restrict__ count = q.count + FE_COUNT_CANDIDATES;
     int n = min(*count, capacity);
     int npad = 1;
     while (npad < n) npad <<= 1;
@@ -663,12 +663,12 @@ __global__ void __launch_bounds__(32) gftt_select_kernel(const FeSeq* __restrict
     const FeSeq& q = seqs[blockIdx.x];
     if (!q.detect) return;
     const unsigned long long* __restrict__ keys = q.keys;
-    const int* __restrict__ count = q.count;
+    const int* __restrict__ count = q.count + FE_COUNT_CANDIDATES;
     const int max_corners = q.max_corners;
     int* __restrict__ cell_cnt = q.cell_cnt;
     short2* __restrict__ cell_pts = q.cell_pts;
     float* __restrict__ out_pts = q.new_pts;
-    int* __restrict__ out_n = q.count + 1;
+    int* __restrict__ out_n = q.count + FE_COUNT_SELECTED;
     const int lane = threadIdx.x;
     const int n = min(*count, capacity);
     for (int i = lane; i < gw * gh; i += 32) cell_cnt[i] = 0;

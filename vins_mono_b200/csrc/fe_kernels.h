@@ -11,6 +11,9 @@ namespace vb {
 
 constexpr int MAX_PYR_LEVELS = 5;
 constexpr int SORT_SMEM_KEYS = 16384;  // 128 KB of 64-bit candidate keys sorted inside one CTA's shared memory
+// A member's counter slot (FeSeq::count, FE_COUNT_SLOT ints): Shi-Tomasi candidates found, corners selected, and the
+// maximum of the min-eigenvalue map as a sortable unsigned (FeSeq::maxv points at it)
+enum : int { FE_COUNT_CANDIDATES = 0, FE_COUNT_SELECTED = 1, FE_COUNT_MAXV = 2, FE_COUNT_SLOT = 4 };
 
 struct PyramidView {
     const uint8_t* img[MAX_PYR_LEVELS];
@@ -38,8 +41,8 @@ struct FeSeq {  // one member's work of one image step
     const int* centres;      // n_centres x 2 kept tracks (rounded)
     float* eig;
     unsigned long long* keys;
-    int* count;              // [0] candidates, [1] selected
-    unsigned* maxv;
+    int* count;              // counter slot: [FE_COUNT_CANDIDATES], [FE_COUNT_SELECTED]
+    unsigned* maxv;          // count + FE_COUNT_MAXV
     int* cell_cnt;
     short2* cell_pts;
     float* new_pts;          // max_corners x 2

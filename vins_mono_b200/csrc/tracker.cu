@@ -31,6 +31,7 @@
 #include "fm_ransac.h"
 #include "hostpool.h"
 #include "kprof.h"
+#include "cuda_check.h"
 #include "vinsb200/tracker.h"
 
 namespace {
@@ -45,6 +46,47 @@ struct DevicePyramid {
 };
 
 inline int cv_round(float v) { return (int)lrintf(v); }
+
+// The batch's point arenas (byte offsets), S members of `cap` points each.  up, host to device: pts_in (S x cap x 2 f32)
+// | centres (S x cap x 2 i32).  down, device to host: pts_out (S x cap x 2 f32) | status (S x cap) | counts (S x
+// FE_COUNT_SLOT i32, 16-byte aligned) | new_pts (S x cap x 2 f32).  The tracking part of each arena comes first, so a
+// frame copies only what its phases produced.
+struct ArenaLayout {
+    size_t cap;
+    size_t centres, up_bytes;                              // up arena; pts_in at 0
+    size_t status, track_bytes, counts, new_pts, dn_bytes;  // down arena; pts_out at 0
+};
+ArenaLayout arena_layout(size_t S, size_t cap) {
+    ArenaLayout a{};
+    a.cap = cap;
+    a.centres = S * cap * 2 * sizeof(float);
+    a.up_bytes = a.centres + S * cap * 2 * sizeof(int);
+    a.status = S * cap * 2 * sizeof(float);
+    a.track_bytes = a.status + S * cap;
+    a.counts = (a.track_bytes + 15) & ~(size_t)15;
+    a.new_pts = a.counts + S * vb::FE_COUNT_SLOT * sizeof(int);
+    a.dn_bytes = a.new_pts + S * cap * 2 * sizeof(float);
+    return a;
+}
+struct ArenaSlots {  // one member's slots in the arenas at one pair of base addresses (pinned host or device)
+    float* pts_in;
+    int* centres;
+    float* pts_out;
+    uint8_t* status;
+    int* counts;
+    float* new_pts;
+};
+ArenaSlots arena_slots(const ArenaLayout& a, uint8_t* up, uint8_t* dn, int k) {
+    const size_t cap = a.cap;
+    ArenaSlots s;
+    s.pts_in = reinterpret_cast<float*>(up) + k * cap * 2;
+    s.centres = reinterpret_cast<int*>(up + a.centres) + k * cap * 2;
+    s.pts_out = reinterpret_cast<float*>(dn) + k * cap * 2;
+    s.status = dn + a.status + k * cap;
+    s.counts = reinterpret_cast<int*>(dn + a.counts) + (size_t)k * vb::FE_COUNT_SLOT;
+    s.new_pts = reinterpret_cast<float*>(dn + a.new_pts) + k * cap * 2;
+    return s;
+}
 
 }  // namespace
 
@@ -68,12 +110,7 @@ struct vt_tracker {
     // this member's slots in the batch arenas
     uint8_t* d_raw = nullptr;  // frame slot (host-image path)
     uint8_t* h_img = nullptr;
-    float* h_pts_in = nullptr;   // pinned, up arena
-    int* h_centres = nullptr;
-    float* h_pts_out = nullptr;  // pinned, down arena
-    uint8_t* h_status = nullptr;
-    int* h_counts = nullptr;
-    float* h_new_pts = nullptr;
+    ArenaSlots h{}, d{};  // in the pinned arenas and in their device copies
     std::vector<int> halfw;
     int capacity = 0;
     // FeatureTracker state (feature_tracker.h:45-64)
@@ -108,11 +145,11 @@ struct vt_batch {
     int raw_pitch = 0, capacity = 0, nlev = 0;
     uint8_t* d_raw = nullptr;   // S x rows x raw_pitch
     uint8_t* h_img = nullptr;   // pinned S x rows x cols
-    uint8_t* h_up = nullptr;    // pinned: pts_in (S x cap x 2 f32) | centres (S x cap x 2 i32)
+    ArenaLayout ar{};
+    uint8_t* h_up = nullptr;    // pinned up arena
     uint8_t* d_up = nullptr;
-    uint8_t* h_dn = nullptr;    // pinned: pts_out (S x cap x 2 f32) | status (S x cap) | counts (S x 2 i32) | new_pts (S x cap x 2 f32)
+    uint8_t* h_dn = nullptr;    // pinned down arena
     uint8_t* d_dn = nullptr;
-    size_t up_pts_bytes = 0, up_bytes = 0, dn_track_bytes = 0, dn_counts_off = 0, dn_bytes = 0;
     int* d_halfw = nullptr;
     vb::KernelProfile prof;  // 0 clahe_lut+apply, 1 pyrdown x3, 2 lk, 3 mask, 4 min_eig, 5 candidates+sort+select
     vb::HostPool* pool = nullptr;
@@ -121,15 +158,6 @@ struct vt_batch {
 };
 
 namespace {
-
-#define VT_CUDA(call)                                                                       \
-    do {                                                                                    \
-        cudaError_t e_ = (call);                                                            \
-        if (e_ != cudaSuccess) {                                                            \
-            t->err = std::string(#call) + ": " + cudaGetErrorString(e_);                    \
-            return VT_ERR_CUDA;                                                             \
-        }                                                                                   \
-    } while (0)
 
 int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
@@ -159,7 +187,7 @@ int alloc_pyramid(vt_tracker* t, DevicePyramid& p) {
         c = (c + 1) / 2;
     }
     p.view.nlev = nlev;
-    VT_CUDA(cudaMalloc(&p.base, total));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMalloc(&p.base, total));
     for (int l = 0; l <= nlev; l++) p.view.img[l] = p.base + offs[l];
     for (int l = nlev + 1; l < vb::MAX_PYR_LEVELS; l++) p.view.img[l] = nullptr;
     return VT_OK;
@@ -332,15 +360,15 @@ int set_mask(vt_tracker* t) {
         bool free_px = true;
         if (t->cfg.fisheye && t->cfg.fisheye_mask) free_px = t->cfg.fisheye_mask[(size_t)py * t->cfg.cols + px] == 255;
         for (int k = 0; k < kept && free_px; k++) {
-            const int dy = std::abs(py - t->h_centres[2 * k + 1]), dx = std::abs(px - t->h_centres[2 * k]);
+            const int dy = std::abs(py - t->h.centres[2 * k + 1]), dx = std::abs(px - t->h.centres[2 * k]);
             if (dy <= r && dx <= t->halfw[dy]) free_px = false;
         }
         if (free_px) {
             t->forw_pts.push_back(it.second.first);
             t->ids.push_back(it.second.second);
             t->track_cnt.push_back(it.first);
-            t->h_centres[2 * kept] = px;
-            t->h_centres[2 * kept + 1] = py;
+            t->h.centres[2 * kept] = px;
+            t->h.centres[2 * kept + 1] = py;
             kept++;
         }
     }
@@ -416,11 +444,11 @@ void step_prepare(vt_tracker* t, const ImageMsg& m, size_t stride, bool on_devic
     t->forw_pts.clear();
     const int n = t->step_first ? 0 : (int)t->cur_pts.size();
     t->step_n = n;
-    if (n) std::memcpy(t->h_pts_in, t->cur_pts.data(), (size_t)n * sizeof(Pt));
+    if (n) std::memcpy(t->h.pts_in, t->cur_pts.data(), (size_t)n * sizeof(Pt));
     q.n_pts = n;
-    q.pts_in = reinterpret_cast<const float*>(b->d_up + ((uint8_t*)t->h_pts_in - b->h_up));
-    q.pts_out = reinterpret_cast<float*>(b->d_dn + ((uint8_t*)t->h_pts_out - b->h_dn));
-    q.status = b->d_dn + (t->h_status - b->h_dn);
+    q.pts_in = t->d.pts_in;
+    q.pts_out = t->d.pts_out;
+    q.status = t->d.status;
     t->h2d_bytes += (size_t)n * sizeof(Pt) + sizeof(vb::FeSeq);
     t->d2h_bytes += (size_t)n * (sizeof(Pt) + 1);
 }
@@ -432,13 +460,13 @@ void step_after_track(vt_tracker* t) {
     q.track = 0;
     const int n = t->step_n;
     if (n) {
-        t->forw_pts.assign(reinterpret_cast<Pt*>(t->h_pts_out), reinterpret_cast<Pt*>(t->h_pts_out) + n);
+        t->forw_pts.assign(reinterpret_cast<Pt*>(t->h.pts_out), reinterpret_cast<Pt*>(t->h.pts_out) + n);
         // status already includes the inBorder() cull (fused into the LK kernel)
-        compact(t->cur_pts, t->h_status);
-        compact(t->forw_pts, t->h_status);
-        compact(t->ids, t->h_status);
-        compact(t->cur_un_pts, t->h_status);
-        compact(t->track_cnt, t->h_status);
+        compact(t->cur_pts, t->h.status);
+        compact(t->forw_pts, t->h.status);
+        compact(t->ids, t->h.status);
+        compact(t->cur_un_pts, t->h.status);
+        compact(t->track_cnt, t->h.status);
     }
     for (auto& c : t->track_cnt) c++;
     t->n_pts.clear();
@@ -457,14 +485,14 @@ void step_after_track(vt_tracker* t) {
     q.n_centres = kept;
     q.mask = t->d_mask;
     q.mask_init = t->cfg.fisheye ? t->d_fisheye : nullptr;
-    q.centres = reinterpret_cast<const int*>(b->d_up + ((uint8_t*)t->h_centres - b->h_up));
+    q.centres = t->d.centres;
     q.eig = t->d_eig;
     q.keys = t->d_keys;
-    q.count = reinterpret_cast<int*>(b->d_dn + ((uint8_t*)t->h_counts - b->h_dn));
-    q.maxv = reinterpret_cast<unsigned*>(q.count + 2);  // the third int of the member's counter slot
+    q.count = t->d.counts;
+    q.maxv = reinterpret_cast<unsigned*>(t->d.counts + vb::FE_COUNT_MAXV);
     q.cell_cnt = t->d_cell_cnt;
     q.cell_pts = t->d_cell_pts;
-    q.new_pts = reinterpret_cast<float*>(b->d_dn + ((uint8_t*)t->h_new_pts - b->h_dn));
+    q.new_pts = t->d.new_pts;
     q.max_corners = n_max_cnt;
     t->h2d_bytes += (size_t)kept * 2 * sizeof(int) + sizeof(vb::FeSeq);
     t->d2h_bytes += 4 * sizeof(int) + (size_t)n_max_cnt * 2 * sizeof(float);
@@ -474,12 +502,12 @@ void step_after_track(vt_tracker* t) {
 // feature_tracker_node.cpp:103-111).
 void step_finish(vt_tracker* t) {
     if (t->step_detect) {
-        if (t->h_counts[0] > t->key_capacity) {
+        if (t->h.counts[vb::FE_COUNT_CANDIDATES] > t->key_capacity) {
             t->err = "Shi-Tomasi candidate buffer overflow";
             t->status = VT_ERR_CAPACITY;
         } else {
-            const int n_new = t->h_counts[1];
-            for (int i = 0; i < n_new; i++) t->n_pts.push_back(Pt{t->h_new_pts[2 * i], t->h_new_pts[2 * i + 1]});
+            const int n_new = t->h.counts[vb::FE_COUNT_SELECTED];
+            for (int i = 0; i < n_new; i++) t->n_pts.push_back(Pt{t->h.new_pts[2 * i], t->h.new_pts[2 * i + 1]});
         }
     }
     if (t->step_pub)
@@ -497,15 +525,6 @@ void step_finish(vt_tracker* t) {
     t->step_active = false;
 }
 
-#define VTB_CUDA(call)                                                       \
-    do {                                                                     \
-        cudaError_t e_ = (call);                                             \
-        if (e_ != cudaSuccess) {                                             \
-            b->err = std::string(#call) + ": " + cudaGetErrorString(e_);     \
-            return VT_ERR_CUDA;                                              \
-        }                                                                    \
-    } while (0)
-
 vb::FeShape base_shape(const vt_batch* b) {
     vb::FeShape sh{};
     sh.S = b->S;
@@ -519,7 +538,7 @@ vb::FeShape base_shape(const vt_batch* b) {
 
 // readImage for every member with msgs[k].active: all of them advance by one image together.
 int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_device) {
-    VTB_CUDA(cudaSetDevice(b->cfg.device));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaSetDevice(b->cfg.device));
     const int S = b->S;
     static const bool trace = std::getenv("VINSB200_TRACE") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
@@ -548,18 +567,18 @@ int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_d
     }
     if (!sh.any_track) return VT_OK;
     const auto t1 = now();
-    VTB_CUDA(cudaEventRecord(b->ev0, b->stream));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaEventRecord(b->ev0, b->stream));
     if (!on_device) {  // the frames of members first_active..last_active travel in one copy
         const int rows = b->cfg.rows, cols = b->cfg.cols;
-        VTB_CUDA(cudaMemcpy2DAsync(b->d_raw + (size_t)first_active * rows * b->raw_pitch, b->raw_pitch,
+        VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpy2DAsync(b->d_raw + (size_t)first_active * rows * b->raw_pitch, b->raw_pitch,
                                    b->h_img + (size_t)first_active * rows * cols, cols, cols, (size_t)rows * (last_active - first_active + 1),
                                    cudaMemcpyHostToDevice, b->stream));
     }
-    VTB_CUDA(cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * S, cudaMemcpyHostToDevice, b->stream));
-    if (sh.max_pts > 0) VTB_CUDA(cudaMemcpyAsync(b->d_up, b->h_up, b->up_pts_bytes, cudaMemcpyHostToDevice, b->stream));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * S, cudaMemcpyHostToDevice, b->stream));
+    if (sh.max_pts > 0) VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->d_up, b->h_up, b->ar.centres, cudaMemcpyHostToDevice, b->stream));
     vb::launch_track(b->d_seq, sh, b->stream, &b->last_launches, &b->prof);
-    if (sh.max_pts > 0) VTB_CUDA(cudaMemcpyAsync(b->h_dn, b->d_dn, b->dn_track_bytes, cudaMemcpyDeviceToHost, b->stream));
-    VTB_CUDA(cudaStreamSynchronize(b->stream));
+    if (sh.max_pts > 0) VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->h_dn, b->d_dn, b->ar.track_bytes, cudaMemcpyDeviceToHost, b->stream));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaStreamSynchronize(b->stream));
     const auto t2 = now();
     b->pool->run(S, [&](int k) {
         if (b->members[k]->step_active) step_after_track(b->members[k]);
@@ -572,18 +591,18 @@ int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_d
         sh.max_centres = std::max(sh.max_centres, q.n_centres);
     }
     if (sh.any_detect) {
-        VTB_CUDA(cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * S, cudaMemcpyHostToDevice, b->stream));
+        VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * S, cudaMemcpyHostToDevice, b->stream));
         if (sh.max_centres > 0)
-            VTB_CUDA(cudaMemcpyAsync(b->d_up + b->up_pts_bytes, b->h_up + b->up_pts_bytes, b->up_bytes - b->up_pts_bytes,
+            VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->d_up + b->ar.centres, b->h_up + b->ar.centres, b->ar.up_bytes - b->ar.centres,
                                      cudaMemcpyHostToDevice, b->stream));
         vb::launch_detect(b->d_seq, sh, b->d_halfw, b->stream, &b->last_launches, &b->prof);
-        VTB_CUDA(cudaMemcpyAsync(b->h_dn + b->dn_counts_off, b->d_dn + b->dn_counts_off, b->dn_bytes - b->dn_counts_off,
+        VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpyAsync(b->h_dn + b->ar.counts, b->d_dn + b->ar.counts, b->ar.dn_bytes - b->ar.counts,
                                  cudaMemcpyDeviceToHost, b->stream));
     }
-    VTB_CUDA(cudaEventRecord(b->ev1, b->stream));
-    VTB_CUDA(cudaEventSynchronize(b->ev1));
-    VTB_CUDA(cudaGetLastError());
-    VTB_CUDA(cudaEventElapsedTime(&b->last_ms, b->ev0, b->ev1));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaEventRecord(b->ev1, b->stream));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaEventSynchronize(b->ev1));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaGetLastError());
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaEventElapsedTime(&b->last_ms, b->ev0, b->ev1));
     const auto t4 = now();
     b->pool->run(S, [&](int k) {
         if (b->members[k]->step_active) step_finish(b->members[k]);
@@ -688,15 +707,10 @@ vt_tracker* create_member(vt_batch* b, int k) {
         return nullptr;
     }
     t->halfw = disc_half_widths(cfg->min_dist);
-    const size_t cap = (size_t)b->capacity, S = (size_t)b->S;
     t->d_raw = b->d_raw + (size_t)k * rows * b->raw_pitch;
     t->h_img = b->h_img + (size_t)k * npx;
-    t->h_pts_in = reinterpret_cast<float*>(b->h_up) + (size_t)k * cap * 2;
-    t->h_centres = reinterpret_cast<int*>(b->h_up + b->up_pts_bytes) + (size_t)k * cap * 2;
-    t->h_pts_out = reinterpret_cast<float*>(b->h_dn) + (size_t)k * cap * 2;
-    t->h_status = b->h_dn + S * cap * 2 * sizeof(float) + (size_t)k * cap;
-    t->h_counts = reinterpret_cast<int*>(b->h_dn + b->dn_counts_off) + (size_t)k * 4;
-    t->h_new_pts = reinterpret_cast<float*>(b->h_dn + b->dn_counts_off + S * 4 * sizeof(int)) + (size_t)k * cap * 2;
+    t->h = arena_slots(b->ar, b->h_up, b->h_dn, k);
+    t->d = arena_slots(b->ar, b->d_up, b->d_dn, k);
     return t;
 }
 
@@ -722,38 +736,28 @@ int vt_batch_create(const vt_config* cfg, int n, vt_batch** out) {
         vt_batch_destroy(b);
         return code;
     };
-#define VT_TRY(call)                                         \
-    do {                                                     \
-        if ((call) != cudaSuccess) return fail(VT_ERR_CUDA); \
-    } while (0)
-    VT_TRY(cudaSetDevice(cfg->device));
-    VT_TRY(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
-    VT_TRY(cudaEventCreate(&b->ev0));
-    VT_TRY(cudaEventCreate(&b->ev1));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaSetDevice(cfg->device));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaEventCreate(&b->ev0));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaEventCreate(&b->ev1));
     const int rows = cfg->rows, cols = cfg->cols;
     const size_t npx = (size_t)rows * cols, S = (size_t)n;
     b->raw_pitch = align_up(cols, 64);
     b->capacity = std::max(cfg->max_cnt, 16);
     b->nlev = lk_levels(rows, cols, 21, 3);
-    const size_t cap = (size_t)b->capacity;
-    b->up_pts_bytes = S * cap * 2 * sizeof(float);
-    b->up_bytes = b->up_pts_bytes + S * cap * 2 * sizeof(int);
-    b->dn_track_bytes = S * cap * 2 * sizeof(float) + S * cap;
-    b->dn_counts_off = (b->dn_track_bytes + 15) & ~(size_t)15;
-    b->dn_bytes = b->dn_counts_off + S * 4 * sizeof(int) + S * cap * 2 * sizeof(float);
-    VT_TRY(cudaMalloc(&b->d_raw, S * rows * b->raw_pitch));
-    VT_TRY(cudaHostAlloc(&b->h_img, S * npx, cudaHostAllocDefault));
-    VT_TRY(cudaMalloc(&b->d_up, b->up_bytes));
-    VT_TRY(cudaHostAlloc(&b->h_up, b->up_bytes, cudaHostAllocDefault));
-    VT_TRY(cudaMalloc(&b->d_dn, b->dn_bytes));
-    VT_TRY(cudaHostAlloc(&b->h_dn, b->dn_bytes, cudaHostAllocDefault));
-    VT_TRY(cudaMalloc(&b->d_seq, sizeof(vb::FeSeq) * S));
-    VT_TRY(cudaHostAlloc(&b->h_seq, sizeof(vb::FeSeq) * S, cudaHostAllocDefault));
+    b->ar = arena_layout(S, (size_t)b->capacity);
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_raw, S * rows * b->raw_pitch));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_img, S * npx, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_up, b->ar.up_bytes));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_up, b->ar.up_bytes, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_dn, b->ar.dn_bytes));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_dn, b->ar.dn_bytes, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_seq, sizeof(vb::FeSeq) * S));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_seq, sizeof(vb::FeSeq) * S, cudaHostAllocDefault));
     std::memset(b->h_seq, 0, sizeof(vb::FeSeq) * S);
     const std::vector<int> hw = disc_half_widths(cfg->min_dist);
-    VT_TRY(cudaMalloc(&b->d_halfw, hw.size() * sizeof(int)));
-    VT_TRY(cudaMemcpy(b->d_halfw, hw.data(), hw.size() * sizeof(int), cudaMemcpyHostToDevice));
-#undef VT_TRY
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_halfw, hw.size() * sizeof(int)));
+    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMemcpy(b->d_halfw, hw.data(), hw.size() * sizeof(int), cudaMemcpyHostToDevice));
     for (int k = 0; k < n; k++) {
         vt_tracker* t = create_member(b, k);
         if (!t) return fail(VT_ERR_CUDA);
@@ -984,8 +988,8 @@ int vt_debug_equalized(vt_tracker* t, int level, uint8_t* out, int* rows, int* c
     if (!t || !t->have_img) return VT_ERR_INVALID;
     const vb::PyramidView& v = t->pyr[t->cur].view;
     if (level < 0 || level > v.nlev) return VT_ERR_INVALID;
-    VT_CUDA(cudaSetDevice(t->cfg.device));
-    VT_CUDA(cudaMemcpy2D(out, v.cols[level], v.img[level], v.pitch[level], v.cols[level], v.rows[level],
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaSetDevice(t->cfg.device));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpy2D(out, v.cols[level], v.img[level], v.pitch[level], v.cols[level], v.rows[level],
                          cudaMemcpyDeviceToHost));
     if (rows) *rows = v.rows[level];
     if (cols) *cols = v.cols[level];
@@ -996,13 +1000,13 @@ int vt_debug_gftt(vt_tracker* t, const uint8_t* img, size_t row_stride, const ui
                   float* corners, int* n_candidates, float* eig_out) {
     if (!t || !img || max_corners <= 0 || max_corners > t->capacity) return VT_ERR_INVALID;
     vt_batch* b = t->batch;
-    VT_CUDA(cudaSetDevice(t->cfg.device));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaSetDevice(t->cfg.device));
     const int rows = t->cfg.rows, cols = t->cfg.cols;
     uint8_t* d_user_mask = nullptr;
-    VT_CUDA(cudaMemcpy2DAsync(t->d_raw, b->raw_pitch, img, row_stride, cols, rows, cudaMemcpyHostToDevice, b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpy2DAsync(t->d_raw, b->raw_pitch, img, row_stride, cols, rows, cudaMemcpyHostToDevice, b->stream));
     if (mask) {
-        VT_CUDA(cudaMalloc(&d_user_mask, (size_t)rows * cols));
-        VT_CUDA(cudaMemcpyAsync(d_user_mask, mask, (size_t)rows * cols, cudaMemcpyHostToDevice, b->stream));
+        VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMalloc(&d_user_mask, (size_t)rows * cols));
+        VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(d_user_mask, mask, (size_t)rows * cols, cudaMemcpyHostToDevice, b->stream));
     }
     vb::FeSeq& q = b->h_seq[t->member];
     std::memset(&q, 0, sizeof(q));
@@ -1014,29 +1018,29 @@ int vt_debug_gftt(vt_tracker* t, const uint8_t* img, size_t row_stride, const ui
     q.mask_init = d_user_mask;
     q.eig = t->d_eig;
     q.keys = t->d_keys;
-    q.count = reinterpret_cast<int*>(b->d_dn + ((uint8_t*)t->h_counts - b->h_dn));
-    q.maxv = reinterpret_cast<unsigned*>(q.count + 2);
+    q.count = t->d.counts;
+    q.maxv = reinterpret_cast<unsigned*>(t->d.counts + vb::FE_COUNT_MAXV);
     q.cell_cnt = t->d_cell_cnt;
     q.cell_pts = t->d_cell_pts;
-    q.new_pts = reinterpret_cast<float*>(b->d_dn + ((uint8_t*)t->h_new_pts - b->h_dn));
+    q.new_pts = t->d.new_pts;
     q.max_corners = max_corners;
-    VT_CUDA(cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * b->S, cudaMemcpyHostToDevice, b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * b->S, cudaMemcpyHostToDevice, b->stream));
     vb::FeShape sh = base_shape(b);
     sh.any_detect = 1;
     vb::launch_detect(b->d_seq, sh, b->d_halfw, b->stream, nullptr, nullptr);
-    VT_CUDA(cudaMemcpyAsync(b->h_dn + b->dn_counts_off, b->d_dn + b->dn_counts_off, b->dn_bytes - b->dn_counts_off,
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(b->h_dn + b->ar.counts, b->d_dn + b->ar.counts, b->ar.dn_bytes - b->ar.counts,
                             cudaMemcpyDeviceToHost, b->stream));
-    VT_CUDA(cudaStreamSynchronize(b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaStreamSynchronize(b->stream));
     q.detect = 0;
     if (d_user_mask) cudaFree(d_user_mask);
-    if (t->h_counts[0] > t->key_capacity) {
+    if (t->h.counts[vb::FE_COUNT_CANDIDATES] > t->key_capacity) {
         t->err = "Shi-Tomasi candidate buffer overflow";
         return VT_ERR_CAPACITY;
     }
-    const int n = t->h_counts[1];
-    if (n_candidates) *n_candidates = t->h_counts[0];
-    std::memcpy(corners, t->h_new_pts, (size_t)n * 2 * sizeof(float));
-    if (eig_out) VT_CUDA(cudaMemcpy(eig_out, t->d_eig, (size_t)rows * cols * sizeof(float), cudaMemcpyDeviceToHost));
+    const int n = t->h.counts[vb::FE_COUNT_SELECTED];
+    if (n_candidates) *n_candidates = t->h.counts[vb::FE_COUNT_CANDIDATES];
+    std::memcpy(corners, t->h.new_pts, (size_t)n * 2 * sizeof(float));
+    if (eig_out) VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpy(eig_out, t->d_eig, (size_t)rows * cols * sizeof(float), cudaMemcpyDeviceToHost));
     return n;
 }
 
@@ -1044,11 +1048,11 @@ int vt_debug_lk(vt_tracker* t, const uint8_t* prev, const uint8_t* next, size_t 
                 float* next_pts, uint8_t* status) {
     if (!t || !prev || !next || n < 0 || n > t->capacity) return VT_ERR_INVALID;
     vt_batch* b = t->batch;
-    VT_CUDA(cudaSetDevice(t->cfg.device));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaSetDevice(t->cfg.device));
     const int rows = t->cfg.rows, cols = t->cfg.cols;
     for (int k = 0; k < 2; k++) {
         DevicePyramid& p = t->pyr[k];
-        VT_CUDA(cudaMemcpy2DAsync(const_cast<uint8_t*>(p.view.img[0]), p.view.pitch[0], k == 0 ? prev : next, row_stride,
+        VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpy2DAsync(const_cast<uint8_t*>(p.view.img[0]), p.view.pitch[0], k == 0 ? prev : next, row_stride,
                                   cols, rows, cudaMemcpyHostToDevice, b->stream));
     }
     vb::FeSeq& q = b->h_seq[t->member];
@@ -1057,24 +1061,24 @@ int vt_debug_lk(vt_tracker* t, const uint8_t* prev, const uint8_t* next, size_t 
     q.cur = t->pyr[0].view;
     q.forw = t->pyr[1].view;
     q.n_pts = n;
-    q.pts_in = reinterpret_cast<const float*>(b->d_up + ((uint8_t*)t->h_pts_in - b->h_up));
-    q.pts_out = reinterpret_cast<float*>(b->d_dn + ((uint8_t*)t->h_pts_out - b->h_dn));
-    q.status = b->d_dn + (t->h_status - b->h_dn);
-    if (n) std::memcpy(t->h_pts_in, pts, (size_t)n * 2 * sizeof(float));
-    VT_CUDA(cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * b->S, cudaMemcpyHostToDevice, b->stream));
-    VT_CUDA(cudaMemcpyAsync(b->d_up, b->h_up, b->up_pts_bytes, cudaMemcpyHostToDevice, b->stream));
+    q.pts_in = t->d.pts_in;
+    q.pts_out = t->d.pts_out;
+    q.status = t->d.status;
+    if (n) std::memcpy(t->h.pts_in, pts, (size_t)n * 2 * sizeof(float));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(b->d_seq, b->h_seq, sizeof(vb::FeSeq) * b->S, cudaMemcpyHostToDevice, b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(b->d_up, b->h_up, b->ar.centres, cudaMemcpyHostToDevice, b->stream));
     vb::FeShape sh = base_shape(b);
     sh.any_track = 1;
     sh.max_pts = n;
     vb::launch_pyramid_only(b->d_seq, sh, 1, b->stream);
     vb::launch_pyramid_only(b->d_seq, sh, 0, b->stream);
     vb::launch_lk_only(b->d_seq, sh, b->stream);
-    VT_CUDA(cudaMemcpyAsync(b->h_dn, b->d_dn, b->dn_track_bytes, cudaMemcpyDeviceToHost, b->stream));
-    VT_CUDA(cudaStreamSynchronize(b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(b->h_dn, b->d_dn, b->ar.track_bytes, cudaMemcpyDeviceToHost, b->stream));
+    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaStreamSynchronize(b->stream));
     q.track = 0;
     if (n) {
-        std::memcpy(next_pts, t->h_pts_out, (size_t)n * 2 * sizeof(float));
-        std::memcpy(status, t->h_status, n);
+        std::memcpy(next_pts, t->h.pts_out, (size_t)n * 2 * sizeof(float));
+        std::memcpy(status, t->h.status, n);
     }
     t->have_img = false;  // the pyramids no longer belong to the tracking state
     return VT_OK;
