@@ -646,6 +646,59 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
         "r"(parity)
         : "memory");
 }
+// Generic-proxy stores of this thread to global memory are ordered before later async-proxy (bulk copy) reads of the same
+// addresses.  Every thread that wrote Spk runs it before the barrier that precedes a bulk copy of Spk in the same kernel.
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// cp.async.bulk moves multiples of 16 bytes: an odd count is rounded up, the extra double lands on Lp[D (D + 1) / 2] (the first
+// entry of the right-hand-side row, written after the transfer has completed; Spk has BA_SPK_SLACK behind the largest D)
+__device__ __forceinline__ unsigned spk_copy_bytes(int D) { return (unsigned)((((D * (D + 1) / 2) + 1) & ~1) * sizeof(double)); }
+
+// Loads the regularised reduced system of the step into the packed array Lp (D + 1 rows): p.Spk + mu E with
+// E = p.diag^2 / p.scale^2 on the diagonal, and p.gred as row D (the right-hand side the factorisation carries along).
+// bulk: Lp is in shared memory and arrives by the bulk copy completing on `bar`; copy_in_flight says the caller has issued
+// that copy already (it is cleared here), otherwise it is issued here (a retry with a larger mu).  Without bulk, Lp (shared
+// or global) is filled with plain loads.  Ends on a barrier.
+__device__ __forceinline__ void step_load_system(const BaProblem& p, double* Lp, double mu, int D, bool bulk, bool& copy_in_flight,
+                                                 unsigned long long* bar, unsigned& phase) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    if (bulk) {
+        if (!copy_in_flight) {  // a retry with a larger mu: fetch the matrix again
+            __syncthreads();    // every thread is done with the previous contents of Lp
+            if (tid == 0) bulk_g2s_chunked(Lp, p.Spk, spk_copy_bytes(D), 8192u, bar);
+        }
+        copy_in_flight = false;
+        const int npk = D * (D + 1) / 2;
+        double rhs[2];  // row D: the right-hand side (D <= 2 nt), fetched while the transfer runs
+#pragma unroll
+        for (int u = 0; u < 2; u++) rhs[u] = tid + u * nt < D ? p.gred[tid + u * nt] : 0.0;
+        mbar_wait(bar, phase);
+        phase ^= 1;
+#pragma unroll
+        for (int u = 0; u < 2; u++)
+            if (tid + u * nt <= D) Lp[npk + tid + u * nt] = rhs[u];
+    } else {
+        const int npk = D * (D + 1) / 2;
+        for (int idx = tid; idx < npk; idx += nt) Lp[idx] = p.Spk[idx];
+        for (int j = tid; j <= D; j += nt) Lp[npk + j] = j < D ? p.gred[j] : 0.0;  // row D: the right-hand side
+    }
+    __syncthreads();
+    for (int i = tid; i < D; i += nt) {
+        const double s_ = p.scale[i];
+        Lp[(size_t)i * (i + 1) / 2 + i] += mu * (p.diag[i] * p.diag[i]) / (s_ * s_);
+    }
+    __syncthreads();
+}
+
+// After a successful cholesky_packed(Lp, ..., D, ..., D + 1): ysm = (S + mu E)^-1 gred.  Row D of Lp holds L^-1 gred already,
+// so only the backward substitution is left.  Ends on a barrier.
+__device__ __forceinline__ void step_solve(const double* Lp, const double* linv, int D, double* ysm) {
+    const int npk = D * (D + 1) / 2;
+    for (int j = threadIdx.x; j < D; j += blockDim.x) ysm[j] = Lp[npk + j];
+    __syncthreads();
+    chol_solve_packed(Lp, linv, D, ysm, false);
+    __syncthreads();
+}
 
 __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ seqs, int use_smem_chol) {
     extern __shared__ __align__(16) double chol_smem[];  // panel copy (CHOL_NB * CHOL_PS), then the packed factor
@@ -682,15 +735,11 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
     bool linear_ok = true;
     long long c0 = clock64();
 #define STAMP(k) do { if (tid == 0) { const long long c1_ = clock64(); st->clk[k] += c1_ - c0; c0 = c1_; } } while (0)
-    const int npk0 = D * (D + 1) / 2;
-    // cp.async.bulk moves multiples of 16 bytes: an odd count is rounded up, the extra double lands on Lp[npk0] (the first
-    // entry of the right-hand-side row, written after the transfer has completed; Spk has BA_SPK_SLACK behind the largest D)
-    const unsigned copy_bytes = (unsigned)(((npk0 + 1) & ~1) * sizeof(double));
     const bool bulk_ok = use_smem_chol != 0;
     bool copy_in_flight = false;
     if (!st->reuse && bulk_ok) {
         // start the transfer of the packed Schur complement now: it overlaps the scaling / gradient phase below
-        if (tid == 0) bulk_g2s_chunked(Lp, p.Spk, copy_bytes, 8192u, &copy_bar);
+        if (tid == 0) bulk_g2s_chunked(Lp, p.Spk, spk_copy_bytes(D), 8192u, &copy_bar);
         copy_in_flight = true;
     }
     if (!st->reuse) {
@@ -708,32 +757,8 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
         STAMP(0);
         // regularised Gauss-Newton step: (S + mu E_p) y_p = gred, E = diag^2 / scale^2
         linear_ok = false;
-        const int npk = D * (D + 1) / 2;
         while (mu < 1.0) {
-            if (bulk_ok) {
-                if (!copy_in_flight) {  // a retry with a larger mu: fetch the matrix again
-                    __syncthreads();    // every thread is done with the previous contents of Lp
-                    if (tid == 0) bulk_g2s_chunked(Lp, p.Spk, copy_bytes, 8192u, &copy_bar);
-                }
-                copy_in_flight = false;
-                double rhs[2];  // row D: the right-hand side (D <= 2 nt), fetched while the transfer runs
-#pragma unroll
-                for (int u = 0; u < 2; u++) rhs[u] = tid + u * nt < D ? p.gred[tid + u * nt] : 0.0;
-                mbar_wait(&copy_bar, copy_phase);
-                copy_phase ^= 1;
-#pragma unroll
-                for (int u = 0; u < 2; u++)
-                    if (tid + u * nt <= D) Lp[npk + tid + u * nt] = rhs[u];
-            } else {
-                for (int idx = tid; idx < npk; idx += nt) Lp[idx] = p.Spk[idx];
-                for (int j = tid; j <= D; j += nt) Lp[npk + j] = j < D ? p.gred[j] : 0.0;  // row D: the right-hand side
-            }
-            __syncthreads();
-            for (int i = tid; i < D; i += nt) {
-                const double s_ = p.scale[i];
-                Lp[(size_t)i * (i + 1) / 2 + i] += mu * (p.diag[i] * p.diag[i]) / (s_ * s_);
-            }
-            __syncthreads();
+            step_load_system(p, Lp, mu, D, bulk_ok, copy_in_flight, &copy_bar, copy_phase);
             STAMP(2);
             const bool ok_ = cholesky_packed(Lp, chol_smem, D, rdiag, linv, &flag, D + 1);
             STAMP(3);
@@ -744,7 +769,12 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
             mu *= 10.0;
             if (tid == 0) st->retries++;
             __syncthreads();
-            if (mu < 1.0) reduce_single_cta(p, a, mu, first);
+            if (mu < 1.0) {
+                reduce_single_cta(p, a, mu, first);
+                // the next attempt bulk-copies the Spk this CTA has just written with ordinary stores; the kernel boundary
+                // that orders ba_reduce_kernel's stores before the first copy is missing here
+                fence_proxy_async_global();
+            }
         }
         if (copy_in_flight) {  // the loop did not run (mu already at its cap): drain the transfer before leaving
             mbar_wait(&copy_bar, copy_phase);
@@ -752,10 +782,7 @@ __global__ void __launch_bounds__(512) ba_step_kernel(const BaSeq* __restrict__ 
             copy_in_flight = false;
         }
         if (linear_ok) {
-            for (int j = tid; j < D; j += nt) ysm[j] = Lp[npk + j];  // L^-1 gred, carried through the factorisation
-            __syncthreads();
-            chol_solve_packed(Lp, linv, D, ysm, false);
-            __syncthreads();
+            step_solve(Lp, linv, D, ysm);
             STAMP(4);
             for (int j = tid; j < D; j += nt) y[j] = ysm[j];
             // landmark back-substitution, 8 lanes per landmark (4 landmarks per warp in flight: the loop is bound by the
@@ -1109,11 +1136,15 @@ __global__ void __launch_bounds__(128) marg_gather_kernel(const BaSeq* __restric
 
 constexpr int MARG_THREADS = 512;
 
-// doubles of the scratch area Ev: staged landmark rows (2 x 16 x qp) or the n x md products Y and X
+// landmark rows marg_solve_kernel stages per round: 8 when the reduced system lives in global memory (the large windows:
+// with 16, the scratch of the window of 22 frames with extrinsic and td, n = 148, overflows the 227 KB of an H100 CTA)
+__host__ __device__ inline int marg_stage_rows(bool w_in_global) { return w_in_global ? 8 : 16; }
+
+// doubles of the scratch area Ev: staged landmark rows (2 x marg_stage_rows x qp) or the n x md products Y and X
 // (+ a copy of the scaled eigenvectors, n x (n|1), when the reduced system lives in shared memory, i.e. small windows)
 __host__ __device__ inline int marg_scratch_doubles(int md, int n, bool w_in_global) {
     const int q = md + n, qp = (q + 3) & ~3, ldm = md + (md & 1);
-    int a = 32 * qp;
+    int a = 2 * marg_stage_rows(w_in_global) * qp;
     const int b = n * (ldm + md), c = w_in_global ? 0 : n * (n | 1);
     a = a > b ? a : b;
     a = a > c ? a : c;
@@ -1156,11 +1187,11 @@ __global__ void __launch_bounds__(MARG_THREADS) marg_solve_kernel(const BaSeq* _
 #define MSTAMP(k) do { const long long c1_ = clock64(); mclk[k] = c1_ - mc0; mc0 = c1_; } while (0)
     // 1. eliminate the landmark columns (exactly diagonal block): W -= sum_c w_c w_c^T / d_c over the landmarks c.
     //    Register-tiled: a thread owns one 4x4 tile of the upper triangle of W (q = 90 -> 276 tiles) and accumulates
-    //    over ALL landmarks in registers; the landmark rows are staged 16 at a time in shared memory (raw and scaled by
+    //    over ALL landmarks in registers; the landmark rows are staged MCH at a time in shared memory (raw and scaled by
     //    1/d_c, row stride qp = q rounded up to 4 so that a tile operand is two 128-bit loads).  Landmark rows are sparse
     //    (only the observing frames' pose blocks): a tile skips a landmark whose scaled operand is zero.
     const int qp = (q + 3) & ~3, nt4 = qp >> 2, ntile = nt4 * (nt4 + 1) / 2;
-    constexpr int MCH = 16;
+    const int MCH = marg_stage_rows(mp.w_in_global != 0);  // the order of the sums does not depend on it
     double* Wl = Ev;             // MCH x qp raw rows
     double* Ws = Ev + MCH * qp;  // MCH x qp rows scaled by 1 / d_c (0 when d_c <= eps)
     double* invd = tv;           // MCH: 1 / d_c, then b_c in invd + MCH
@@ -1603,6 +1634,27 @@ void launch_eval(const BaSeq* seqs, const BatchShape& sh, int grid, int initial,
     else ba_eval_kernel<false, false><<<g, 32 * LIN_WARPS, 0, s>>>(seqs, initial);
 }
 
+// Schur gather of every member: a CTA per pose-type block pair, incl. the relocalisation pose when a member of this frame has
+// one (CTAs of pairs a member does not have return at once), then the CTAs of the generic entries
+void launch_reduce(const BaSeq* seqs, const BatchShape& sh, cudaStream_t s) {
+    const int NV = sh.W + 1 + (sh.est_ex ? 1 : 0) + (sh.est_td ? 1 : 0) + (sh.any_relo ? 1 : 0), n_pairs = NV * (NV + 1) / 2;
+    const int generic = (sh.D * (sh.D + 1) / 2 + 4 * RED_THREADS - 1) / (4 * RED_THREADS);
+    if (sh.any_relo) ba_reduce_kernel<true><<<dim3(n_pairs + generic, sh.S), RED_THREADS, 0, s>>>(seqs, n_pairs);
+    else ba_reduce_kernel<false><<<dim3(n_pairs + generic, sh.S), RED_THREADS, 0, s>>>(seqs, n_pairs);
+}
+
+// Dynamic shared memory of marg_solve_kernel at the batch's maxima, with the kernel's opt-in on this device raised to it
+size_t prepare_marg_solve(const BatchShape& sh) {
+    const size_t smem = marg_solve_smem_bytes(sh.max_md, sh.max_n, sh.w_in_global != 0);
+    std::lock_guard<std::mutex> lock(g_cfg_mutex);
+    DeviceCfg& c = device_cfg_locked();
+    if ((int)smem > c.marg_configured) {
+        cudaFuncSetAttribute(marg_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        c.marg_configured = (int)smem;
+    }
+    return smem;
+}
+
 }  // namespace
 
 void launch_ba_solve(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* launches, KernelProfile* prof) {
@@ -1613,10 +1665,6 @@ void launch_ba_solve(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* lau
     dmax.L = sh.max_L;
     dmax.W = sh.W;
     const int eval_grid = ba_eval_grid(dmax);
-    // pose-type blocks, incl. the relocalisation pose when a member of this frame has one (CTAs of pairs a member does not
-    // have return at once)
-    const int NV = sh.W + 1 + (sh.est_ex ? 1 : 0) + (sh.est_td ? 1 : 0) + (sh.any_relo ? 1 : 0), n_pairs = NV * (NV + 1) / 2;
-    const int generic = (sh.D * (sh.D + 1) / 2 + 4 * RED_THREADS - 1) / (4 * RED_THREADS);
     const size_t panel_bytes = sizeof(double) * CHOL_NB * CHOL_PS;
     const size_t chol_bytes = sizeof(double) * (size_t)(sh.D + 1) * (sh.D + 2) / 2 + panel_bytes;
     int use_smem;
@@ -1638,8 +1686,7 @@ void launch_ba_solve(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* lau
     n += 1;
     for (int it = 0; it < sh.max_iterations; it++) {
         prof->begin(s);
-        if (sh.any_relo) ba_reduce_kernel<true><<<dim3(n_pairs + generic, sh.S), RED_THREADS, 0, s>>>(seqs, n_pairs);
-        else ba_reduce_kernel<false><<<dim3(n_pairs + generic, sh.S), RED_THREADS, 0, s>>>(seqs, n_pairs);
+        launch_reduce(seqs, sh, s);
         prof->end(1, s);
         prof->begin(s);
         ba_step_kernel<<<sh.S, 512, step_dyn, s>>>(seqs, use_smem);
@@ -1660,15 +1707,7 @@ void launch_marginalize(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* 
     KernelProfile none;
     if (!prof) prof = &none;
     if (!sh.any_marg) return;
-    const size_t smem = marg_solve_smem_bytes(sh.max_md, sh.max_n, sh.w_in_global != 0);
-    {
-        std::lock_guard<std::mutex> lock(g_cfg_mutex);
-        DeviceCfg& c = device_cfg_locked();
-        if ((int)smem > c.marg_configured) {
-            cudaFuncSetAttribute(marg_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            c.marg_configured = (int)smem;
-        }
-    }
+    const size_t smem = prepare_marg_solve(sh);
     const int zgrid = std::max(1, std::min(64, (int)(((size_t)sh.max_P * sh.max_P + 256 * 8 - 1) / (256 * 8))));
     const int egrid = (sh.max_n_lm + LIN_WARPS - 1) / LIN_WARPS + 2;
     const int dense_ctas = 16, lm_ctas = (sh.max_n_lm + 3) / 4;
