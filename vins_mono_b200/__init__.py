@@ -7,3 +7,4 @@ loading fails loudly when the library is missing, creating a tracker fails when 
 from .tracker import FeatureTracker, TrackerBatch, TrackerConfig, load_library, LIB_PATH  # noqa: F401
 from .estimator import Estimator, EstimatorBatch, EstimatorConfig, debug_projection_factor, debug_imu_factor  # noqa: F401
 from .replay import ReplaySession  # noqa: F401
+from .pose_graph import PoseGraph, PoseGraphBatch, PoseGraphError, debug_four_dof_error  # noqa: F401

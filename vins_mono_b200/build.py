@@ -11,7 +11,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libvinsb200.so")
 
 # The front end must reproduce OpenCV's float arithmetic bit for bit: no FMA contraction there.  The back end is
-# double precision checked to a tolerance, so its kernels (ba_*.cu) keep nvcc's default contraction (DFMA).
+# double precision checked to a tolerance, so its kernels (ba_*.cu, and the pose graph's pg_*.cu) keep nvcc's default
+# contraction (DFMA).
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-O2", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
@@ -41,7 +42,7 @@ def build(force=False, verbose=False):
     for src in sources():
         obj = os.path.join(objdir, os.path.basename(src) + ".o")
         objs.append(obj)
-        fmad = "--fmad=true" if os.path.basename(src).startswith("ba_") else "--fmad=false"
+        fmad = "--fmad=true" if os.path.basename(src).startswith(("ba_", "pg_")) else "--fmad=false"
         cmd = ["nvcc", *NVCC_FLAGS, fmad, "-x", "cu", "-c", src, "-o", obj]
         if verbose:
             print(" ".join(cmd))
