@@ -21,8 +21,13 @@
  * by the new drift when the result is collected (pose_graph.cpp:562-571).
  *
  * Plain C, int status (0 ok, < 0 vp_status), no CPU fallback.  A handle is externally synchronised.  Capacity: at most
- * max_keyframes key frames, and at most 88 free loop anchors (4 x 88 = 352 border columns) in an optimised range; a
- * call that would exceed either returns VP_ERR_CAPACITY and leaves the graph as it was.
+ * max_keyframes key frames, and at most max_anchors free loop anchors (distinct older key frames that loop edges land
+ * on) in an optimised range; a call that would exceed either returns VP_ERR_CAPACITY and leaves the graph as it was.
+ * Each anchor adds 4 columns to the dense border of the solve.  Borders up to 352 columns (88 anchors) are factored in
+ * one CTA in shared memory; larger ones over many CTAs in global memory, on the FP64 tensor cores.  The device workspace
+ * grows with max_anchors: per graph about 16 ceil(max_keyframes / 4) (4 max_anchors + 1) doubles for the chain's border
+ * columns, plus (4 max_anchors + 1)^2 rounded up to 64 columns for the border system when max_anchors > 88; at 2048 key
+ * frames and 1024 anchors that is about 268 MB + 138 MB.
  */
 #ifndef VINSB200_POSE_GRAPH_H
 #define VINSB200_POSE_GRAPH_H
@@ -37,6 +42,8 @@ typedef struct vp_config {
     int max_keyframes;       /* key-frame capacity of the graph */
     int fast_relocalization; /* FAST_RELOCALIZATION (pose_graph_node.cpp, euroc_config.yaml:fast_relocalization) */
     int device;
+    int max_anchors;         /* free-loop-anchor capacity of an optimised range: 0 = 88 (today's workspace), or 1 .. 1024;
+                                anything else is VP_ERR_INVALID from vp_create / vp_batch_create */
 } vp_config;
 
 typedef struct vp_graph vp_graph;

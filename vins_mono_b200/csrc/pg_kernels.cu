@@ -8,17 +8,28 @@
 // loop anchor) is constant.  The damped normal equations are solved exactly with this structure:
 //   chain   the free key frames in super-blocks of 4 by local index (16 unknowns each).  Sequential edges reach back at
 //           most 4 key frames, so their part of the system is block-tridiagonal.
-//   border  the free loop anchors (old ends of loop edges), 4 columns each, D <= PG_MAX_D.  Their rows and columns are
+//   border  the free loop anchors (old ends of loop edges), 4 columns each, D of them.  Their rows and columns are
 //           identity rows in the chain; every loop edge has an end in the border or a constant end.
-//   step 1  block Cholesky along the chain (pg_chain_kernel, one CTA per member), carrying W = L^-1 B and y = L^-1 (-g)
-//           as extra right-hand sides, one thread per border column.
-//   step 2  S = C - W^T W and z = -g_b - W^T y (pg_border_kernel, 32 x 32 tiles, rows summed in ascending order; W is a
-//           staircase, each column starts at its first coupled super-block).
-//   step 3  cholesky_packed / chol_solve_packed on [S; z^T], then back-substitution through the chain (pg_solve_kernel).
+//   step 1  block Cholesky along the chain (pg_chain_kernel, ceil((D + 1) / 384) CTAs per member), carrying
+//           W = L^-1 B and y = L^-1 (-g) as extra right-hand sides, one thread per border column.
+//   step 2  S = C - W^T W and z = -g_b - W^T y, rows summed in ascending order; W is a staircase, each column starts at
+//           its first coupled super-block.
+//   step 3  the Cholesky of [S; z^T] (the z row gives the forward solve), the backward solve, then back-substitution
+//           through the chain.
+// Steps 2 and 3 take one of two routes per member, both in the same launch chain (each kernel returns early for the
+// members of the other route):
+//   D <= PG_MAX_D  pg_border_kernel (32 x 32 tiles into the packed system), pg_solve_kernel (cholesky_packed and
+//                  chol_solve_packed in one CTA, in shared memory).
+//   D >  PG_MAX_D  the multi-CTA path, in global memory on U (pg_layout.h): pg_tile_kernel<false> (S and z, one 64 x 64
+//                  tile per CTA on FP64 tensor cores), per panel of 64 columns pg_panel_kernel (diagonal tile and the
+//                  panel's row) and pg_tile_kernel<true> (the trailing update, the same tile product), then
+//                  pg_solve_large_kernel (blocked backward solve and the chain's back-substitution).
 #include "pg_kernels.h"
 #include "pg_layout.h"
 
+#include <algorithm>
 #include <cfloat>
+#include <climits>
 #include <mutex>
 
 #include "ba_device.cuh"
@@ -83,8 +94,9 @@ struct PgView {
     const double *pose, *loopm;
     const int *seq, *loop, *bslot, *lfirst, *lnext, *anchors;
     PgState* st;
-    double *x, *xc, *dx, *scale, *ypr, *smeas, *blk, *g, *L, *F, *W, *Sp;
+    double *x, *xc, *dx, *scale, *ypr, *smeas, *blk, *g, *L, *F, *W, *Sp, *U, *Ud, *yb;
     int* start;
+    int Np;
     double* out;
 };
 
@@ -108,10 +120,12 @@ __device__ PgView pg_view(const PgLaunch& a, int slot) {
     v.lnext = reinterpret_cast<const int*>(in + il.lnext);
     v.anchors = reinterpret_cast<const int*>(in + il.anchors);
     double* w = a.d_work + (size_t)m * a.work_stride;
-    const PgWorkLayout wl = pg_work_layout(a.cap_n);
+    const PgWorkLayout wl = pg_work_layout(a.cap_n, a.cap_anchors);
     v.st = reinterpret_cast<PgState*>(w + wl.state);
     v.x = w + wl.x; v.xc = w + wl.xc; v.dx = w + wl.dx; v.scale = w + wl.scale; v.ypr = w + wl.ypr; v.smeas = w + wl.smeas;
     v.blk = w + wl.blk; v.g = w + wl.g; v.L = w + wl.L; v.F = w + wl.F; v.W = w + wl.W; v.Sp = w + wl.Sp;
+    v.U = w + wl.U; v.Ud = w + wl.Ud; v.yb = w + wl.yb;
+    v.Np = pg_tile_np(v.D);
     v.start = reinterpret_cast<int*>(w + wl.start);
     v.out = a.d_out + reinterpret_cast<const long long*>(a.d_in + h.out_off)[slot];
     return v;
@@ -306,14 +320,17 @@ __device__ __forceinline__ double h_entry(const PgView& v, int ka, int kb, int p
 }
 __device__ __forceinline__ double damped(double h, double radius) { return h + fmin(fmax(h, 1e-6), 1e32) / radius; }
 
-// ---- step 1: block Cholesky along the chain; thread c < D + 1 carries border column c (c = D: the right-hand side)
+// ---- step 1: block Cholesky along the chain; thread c < D + 1 carries border column c (c = D: the right-hand side).
+//      The columns spread over ceil((D + 1) / 384) CTAs (grid.x; grid.y is the member slot).  Every CTA repeats the
+//      super-block factorisation, which is deterministic, so all compute the same bits; CTA 0 alone stores L and F.
 __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
     __shared__ double Lp[16][17], Lc[16][17], Fs[16][17], M[16][17];
     __shared__ int fail;
-    const PgView v = pg_view(a, blockIdx.x);
-    if (v.st->done) return;
+    const PgView v = pg_view(a, blockIdx.y);
+    if (v.st->done || (int)(blockIdx.x * blockDim.x) >= v.Dp) return;
+    const bool writer = blockIdx.x == 0;
     const double radius = v.st->radius;
-    const int tid = threadIdx.x, c = tid;
+    const int tid = threadIdx.x, c = blockIdx.x * blockDim.x + tid;
     const bool col = c < v.Dp;
     int bk = -1, bq = 0;
     if (col && c < v.D) { bk = v.anchors[c >> 2]; bq = c & 3; }
@@ -347,7 +364,7 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
             __syncthreads();
             for (int e = tid; e < 256; e += blockDim.x) {
                 const int r = e >> 4, q = e & 15;
-                v.F[256 * s + e] = Fs[r][q];
+                if (writer) v.F[256 * s + e] = Fs[r][q];
                 if (q <= r) {
                     double acc = 0;
                     for (int t = 0; t < 16; t++) acc += Fs[r][t] * Fs[q][t];
@@ -381,7 +398,7 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
                 for (int q = 0; q < 16; q++) {
                     const double val = q <= r ? row[q] : 0.0;
                     Lc[r][q] = val;
-                    v.L[256 * s + 16 * r + q] = val;
+                    if (writer) v.L[256 * s + 16 * r + q] = val;
                 }
                 if (!ok) fail = 1;
             }
@@ -425,14 +442,14 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
         __syncthreads();
     }
     if (col) v.start[c] = started ? start : v.nsb;
-    if (tid == 0 && fail) v.st->lin_fail = 1;
+    if (writer && tid == 0 && fail) v.st->lin_fail = 1;
 }
 
 // ---- step 2: the border system [S; z^T] packed (row D = z), one 32 x 32 tile per CTA, W rows in ascending order
 __global__ void __launch_bounds__(256) pg_border_kernel(PgLaunch a) {
     __shared__ double Wa[64][33], Wb[64][33];
     const PgView v = pg_view(a, blockIdx.y);
-    if (v.st->done || v.st->lin_fail || v.D == 0) return;
+    if (v.st->done || v.st->lin_fail || v.D == 0 || v.D > PG_MAX_D) return;
     const int T = (v.Dp + 31) / 32, t = blockIdx.x;
     if (t >= T * (T + 1) / 2) return;
     int ti = 0;
@@ -486,26 +503,11 @@ __global__ void __launch_bounds__(256) pg_border_kernel(PgLaunch a) {
     }
 }
 
-// ---- step 3: factor the border system, solve it, back-substitute through the chain; the step (unscaled) into dx
-__global__ void __launch_bounds__(512) pg_solve_kernel(PgLaunch a) {
-    extern __shared__ __align__(16) double pg_panel[];  // CHOL_NB * CHOL_PS
-    __shared__ double rdiag[PG_MAX_D], yb[PG_MAX_D], linv[(PG_MAX_D / CHOL_NB) * 64];
-    __shared__ double Ls[16][17], Fn[16][17], xs[16], xn[16], rhs[16];
-    __shared__ int flag;
-    const PgView v = pg_view(a, blockIdx.x);
-    if (v.st->done || v.st->lin_fail) return;
+// Back-substitution through the chain for a member whose border step yb (scaled) is known: the step (unscaled) into dx.
+// The 16 x 16 blocks and vectors are the caller's shared memory.
+__device__ __forceinline__ void chain_back_substitute(const PgView& v, const double* yb, double (*Ls)[17], double (*Fn)[17], double* xs,
+                                                      double* xn, double* rhs) {
     const int tid = threadIdx.x, D = v.D, Dp = v.Dp;
-    if (D > 0) {
-        const bool ok = cholesky_packed(v.Sp, pg_panel, D, rdiag, linv, &flag, D + 1);
-        if (!ok) {
-            if (tid == 0) v.st->lin_fail = 1;
-            return;
-        }
-        for (int c = tid; c < D; c += blockDim.x) yb[c] = v.Sp[(size_t)D * (D + 1) / 2 + c];
-        __syncthreads();
-        chol_solve_packed(v.Sp, linv, D, yb, false);
-        __syncthreads();
-    }
     if (tid < 16) xn[tid] = 0.0;
     const int wid = tid >> 5, lane = tid & 31;
     for (int s = v.nsb - 1; s >= 0; s--) {
@@ -553,6 +555,226 @@ __global__ void __launch_bounds__(512) pg_solve_kernel(PgLaunch a) {
         }
         __syncthreads();
     }
+}
+
+// ---- step 3: factor the border system, solve it, back-substitute through the chain; the step (unscaled) into dx
+__global__ void __launch_bounds__(512) pg_solve_kernel(PgLaunch a) {
+    extern __shared__ __align__(16) double pg_panel[];  // CHOL_NB * CHOL_PS
+    __shared__ double rdiag[PG_MAX_D], yb[PG_MAX_D], linv[(PG_MAX_D / CHOL_NB) * 64];
+    __shared__ double Ls[16][17], Fn[16][17], xs[16], xn[16], rhs[16];
+    __shared__ int flag;
+    const PgView v = pg_view(a, blockIdx.x);
+    if (v.st->done || v.st->lin_fail || v.D > PG_MAX_D) return;
+    const int tid = threadIdx.x, D = v.D;
+    if (D > 0) {
+        const bool ok = cholesky_packed(v.Sp, pg_panel, D, rdiag, linv, &flag, D + 1);
+        if (!ok) {
+            if (tid == 0) v.st->lin_fail = 1;
+            return;
+        }
+        for (int c = tid; c < D; c += blockDim.x) yb[c] = v.Sp[(size_t)D * (D + 1) / 2 + c];
+        __syncthreads();
+        chol_solve_packed(v.Sp, linv, D, yb, false);
+        __syncthreads();
+    }
+    chain_back_substitute(v, yb, Ls, Fn, xs, xn, rhs);
+}
+
+// ---- the multi-CTA path (D > PG_MAX_D).  U holds the upper triangle of [S z] (z in column D; rows and columns past D
+//      are padding, 1 on the diagonal and 0 elsewhere), PG_TILE x PG_TILE tiles, Np = v.Np columns.  Right-looking
+//      blocked Cholesky U = R^T R, panel p = rows / columns [64 p, 64 p + 64): the diagonal tile's factor goes to Ud, the
+//      panel's row right of it becomes R's (including R^-T z = the forward solve, in column D), and the trailing tiles
+//      are updated by the same tile product that forms S.
+
+// FP64 tensor-core MMA m8n8k4, d = a b + d.  Fragments (PTX ISA, mma.m8n8k4 with .f64): a = A[lane / 4][lane % 4],
+// b = B[lane % 4][lane / 4], d[e] = D[lane / 4][2 (lane % 4) + e].
+__device__ __forceinline__ void mma_f64_m8n8k4(double* d, double a, double b) {
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};\n"
+                 : "+d"(d[0]), "+d"(d[1])
+                 : "d"(a), "d"(b));
+}
+
+constexpr int PG_TK = 32;           // rows of X per shared-memory stage
+constexpr int PG_TS = PG_TILE + 4;  // padded stage row: the fragment loads hit 16 distinct 8-byte banks per half-warp
+
+// acc = X[k0:k1, i0:i0+64]^T X[k0:k1, j0:j0+64] over the rows in ascending order (stages of PG_TK rows, 4 rows per MMA).
+// X is row-major with leading dimension ld; columns >= ncols read as 0, and with kstart != NULL so does every row below
+// 16 kstart[column] (W's staircase: those rows are not written by the chain kernel).  256 threads: warp w owns rows
+// 32 (w / 4) + 8 mt and columns 16 (w % 4) + 8 nt of the tile; acc[mt][nt][e] is its MMA fragment.
+__device__ __forceinline__ void tile_product(const double* X, size_t ld, int k0, int k1, int i0, int j0, int ncols, const int* kstart,
+                                             double (*Xa)[PG_TS], double (*Xb)[PG_TS], double (&acc)[4][2][2]) {
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, lc = tid & (PG_TILE - 1);
+    const int ca = i0 + lc, cb = j0 + lc;
+    const int ka = ca < ncols ? (kstart ? 16 * kstart[ca] : 0) : INT_MAX;
+    const int kb = cb < ncols ? (kstart ? 16 * kstart[cb] : 0) : INT_MAX;
+#pragma unroll
+    for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+        for (int nt = 0; nt < 2; nt++) acc[mt][nt][0] = acc[mt][nt][1] = 0.0;
+    const int m0 = 32 * (w >> 2) + (lane >> 2), n0 = 16 * (w & 3) + (lane >> 2), kl = lane & 3;
+    for (int ch = k0; ch < k1; ch += PG_TK) {
+#pragma unroll
+        for (int q = 0; q < PG_TK * PG_TILE / 256; q++) {
+            const int rr = (tid >> 6) + 4 * q, k = ch + rr;
+            Xa[rr][lc] = (k < k1 && k >= ka) ? X[(size_t)k * ld + ca] : 0.0;
+            Xb[rr][lc] = (k < k1 && k >= kb) ? X[(size_t)k * ld + cb] : 0.0;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < PG_TK; kk += 4) {
+            double fa[4], fb[2];
+#pragma unroll
+            for (int mt = 0; mt < 4; mt++) fa[mt] = Xa[kk + kl][m0 + 8 * mt];
+#pragma unroll
+            for (int nt = 0; nt < 2; nt++) fb[nt] = Xb[kk + kl][n0 + 8 * nt];
+#pragma unroll
+            for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+                for (int nt = 0; nt < 2; nt++) mma_f64_m8n8k4(acc[mt][nt], fa[mt], fb[nt]);
+        }
+        __syncthreads();
+    }
+}
+
+// ---- tiles of U's upper triangle, one per CTA (grid.x; grid.y is the member slot).
+//      kTrailing = false (p unused): U = [C z] - W^T [W y], rows of W from the tile's first coupled super-block on.
+//      kTrailing = true: after panel p, U_IJ -= R_pI^T R_pJ for the tiles p < I <= J.
+template <bool kTrailing>
+__global__ void __launch_bounds__(256) pg_tile_kernel(PgLaunch a, int p) {
+    __shared__ __align__(16) double Xa[PG_TK][PG_TS], Xb[PG_TK][PG_TS];
+    const PgView v = pg_view(a, blockIdx.y);
+    if (v.st->done || v.st->lin_fail || v.D <= PG_MAX_D) return;
+    const int base = kTrailing ? p + 1 : 0, R = v.Np / PG_TILE - base, t = blockIdx.x;
+    if (t >= R * (R + 1) / 2) return;
+    int ti = 0;
+    while ((ti + 1) * (ti + 2) / 2 <= t) ti++;
+    const int i0 = PG_TILE * (base + t - ti * (ti + 1) / 2), j0 = PG_TILE * (base + ti);  // i0 <= j0
+    const size_t Np = v.Np;
+    const int D = v.D, Dp = v.Dp, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    double acc[4][2][2];
+    if (kTrailing) {
+        tile_product(v.U + (size_t)PG_TILE * p * Np, Np, 0, PG_TILE, i0, j0, (int)Np, nullptr, Xa, Xb, acc);
+    } else {
+        int fa = v.nsb, fb = v.nsb;
+        for (int k = 0; k < PG_TILE; k++) {
+            if (i0 + k < Dp) fa = min(fa, v.start[i0 + k]);
+            if (j0 + k < Dp) fb = min(fb, v.start[j0 + k]);
+        }
+        tile_product(v.W, Dp, 16 * max(fa, fb), 16 * v.nsb, i0, j0, Dp, v.start, Xa, Xb, acc);
+    }
+    const double radius = v.st->radius;
+#pragma unroll
+    for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+        for (int nt = 0; nt < 2; nt++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int i = i0 + 32 * (w >> 2) + 8 * mt + (lane >> 2), j = j0 + 16 * (w & 3) + 8 * nt + 2 * (lane & 3) + e;
+                if (i > j) continue;
+                double* u = v.U + (size_t)i * Np + j;
+                if (kTrailing) {
+                    *u -= acc[mt][nt][e];
+                } else if (i < D && j <= D) {
+                    const int ki = v.anchors[i >> 2];
+                    double h;
+                    if (j == D) {
+                        h = -v.g[4 * ki + (i & 3)];
+                    } else {
+                        h = h_entry(v, ki, v.anchors[j >> 2], i & 3, j & 3);
+                        if (i == j) h = damped(h, radius);
+                    }
+                    *u = h - acc[mt][nt][e];
+                } else {
+                    *u = i == j ? 1.0 : 0.0;
+                }
+            }
+}
+
+// ---- panel p: CTA c (grid.x) factors the diagonal tile U_pp = R_pp^T R_pp in shared memory (every CTA, the same bits)
+//      and, for c > 0, solves R_pp^T R_p,p+c = U_p,p+c in place, right-looking by rows.  CTA 0 stores R_pp in Ud (the
+//      other CTAs still read U_pp) and flags a pivot below D that is not positive and finite, as cholesky_packed does;
+//      pivots at and past D (the z column and the padding) are taken as 1.
+constexpr size_t PG_PANEL_SMEM = 2 * sizeof(double) * PG_TILE * (PG_TILE + 1);  // Rd | B, above the 48 KB default
+
+__global__ void __launch_bounds__(256) pg_panel_kernel(PgLaunch a, int p) {
+    extern __shared__ __align__(16) double pg_panel_tiles[];
+    double(*Rd)[PG_TILE + 1] = reinterpret_cast<double(*)[PG_TILE + 1]>(pg_panel_tiles);
+    double(*B)[PG_TILE + 1] = Rd + PG_TILE;
+    __shared__ int bad;
+    const PgView v = pg_view(a, blockIdx.y);
+    if (v.st->done || v.D <= PG_MAX_D) return;
+    const int c = blockIdx.x, tid = threadIdx.x;
+    if (p + c >= v.Np / PG_TILE) return;
+    const size_t Np = v.Np;
+    const double* Upp = v.U + (size_t)PG_TILE * p * Np + PG_TILE * p;
+    double* Ub = v.U + (size_t)PG_TILE * p * Np + PG_TILE * (p + c);
+    for (int e = tid; e < PG_TILE * PG_TILE; e += blockDim.x) {
+        const int r = e / PG_TILE, q = e % PG_TILE;
+        Rd[r][q] = q >= r ? Upp[r * Np + q] : 0.0;
+        if (c) B[r][q] = Ub[r * Np + q];
+    }
+    if (tid == 0) bad = 0;
+    __syncthreads();
+    for (int k = 0; k < PG_TILE; k++) {
+        const double pk = Rd[k][k];
+        const bool real = PG_TILE * p + k < v.D;
+        const double d = real ? sqrt(pk) : 1.0;
+        if (tid == 0 && real && (!(pk > 0.0) || !isfinite(pk))) bad = 1;
+        __syncthreads();
+        for (int j = k + tid; j < PG_TILE; j += blockDim.x) Rd[k][j] = j == k ? d : Rd[k][j] / d;
+        if (c)
+            for (int j = tid; j < PG_TILE; j += blockDim.x) B[k][j] /= d;
+        __syncthreads();
+        for (int e = tid; e < PG_TILE * PG_TILE; e += blockDim.x) {
+            const int i = e / PG_TILE, j = e % PG_TILE;
+            if (i <= k) continue;
+            if (j >= i) Rd[i][j] -= Rd[k][i] * Rd[k][j];
+            if (c) B[i][j] -= Rd[k][i] * B[k][j];
+        }
+        __syncthreads();
+    }
+    if (c) {
+        for (int e = tid; e < PG_TILE * PG_TILE; e += blockDim.x) Ub[(e / PG_TILE) * Np + e % PG_TILE] = B[e / PG_TILE][e % PG_TILE];
+    } else {
+        double* ud = v.Ud + (size_t)PG_TILE * PG_TILE * p;
+        for (int e = tid; e < PG_TILE * PG_TILE; e += blockDim.x) ud[e] = Rd[e / PG_TILE][e % PG_TILE];
+        if (tid == 0 && bad) v.st->lin_fail = 1;
+    }
+}
+
+// ---- step 3 of the multi-CTA path: R x = R^-T z by panels from the last (the rows' sums over the later panels one warp
+//      per row, the diagonal tile by one warp from its last row), x = the border step into yb; then the chain.
+__global__ void __launch_bounds__(512) pg_solve_large_kernel(PgLaunch a) {
+    __shared__ double Rs[PG_TILE][PG_TILE + 1], rs[PG_TILE];
+    __shared__ double Ls[16][17], Fn[16][17], xs[16], xn[16], rhs[16];
+    const PgView v = pg_view(a, blockIdx.x);
+    if (v.st->done || v.st->lin_fail || v.D <= PG_MAX_D) return;
+    const int tid = threadIdx.x, D = v.D, wid = tid >> 5, lane = tid & 31, nw = blockDim.x >> 5;
+    const size_t Np = v.Np;
+    for (int p = (D - 1) / PG_TILE; p >= 0; p--) {
+        const int r0 = PG_TILE * p, nr = min(PG_TILE, D - r0);
+        const double* ud = v.Ud + (size_t)PG_TILE * PG_TILE * p;
+        for (int e = tid; e < PG_TILE * PG_TILE; e += blockDim.x) Rs[e / PG_TILE][e % PG_TILE] = ud[e];
+        __syncthreads();
+        for (int i = wid; i < nr; i += nw) {
+            const double* Ri = v.U + (size_t)(r0 + i) * Np;
+            double part = 0;
+            for (int j = r0 + PG_TILE + lane; j < D; j += 32) part += Ri[j] * v.yb[j];
+            part = warp_sum_d(part);
+            if (lane == 0) rs[i] = (D < r0 + PG_TILE ? Rs[i][D - r0] : Ri[D]) - part;
+        }
+        __syncthreads();
+        if (wid == 0)
+            for (int i = nr - 1; i >= 0; i--) {
+                double part = 0;
+                for (int j = i + 1 + lane; j < nr; j += 32) part += Rs[i][j] * v.yb[r0 + j];
+                part = warp_sum_d(part);
+                if (lane == 0) v.yb[r0 + i] = (rs[i] - part) / Rs[i][i];
+                __syncwarp();
+            }
+        __syncthreads();
+    }
+    chain_back_substitute(v, v.yb, Ls, Fn, xs, xn, rhs);
 }
 
 // ---- update: model cost change, candidate x [+] delta, its cost, the trust-region decision (sfm_bundle's order)
@@ -671,8 +893,8 @@ __global__ void pg_debug_edge_kernel(const double* prm, const double* meas, int 
 }  // namespace
 
 namespace {
-// pg_solve_kernel's dynamic shared memory (the Cholesky panel) is above the 48 KB default together with its static part:
-// the opt-in is a per-device function attribute, set once per device.
+// pg_solve_kernel's dynamic shared memory (the Cholesky panel) is above the 48 KB default together with its static part,
+// and so is pg_panel_kernel's: the opt-in is a per-device function attribute, set once per device.
 std::mutex g_pg_cfg_mutex;
 bool g_pg_configured[64];
 
@@ -683,6 +905,7 @@ cudaError_t configure_device(size_t panel) {
     std::lock_guard<std::mutex> lock(g_pg_cfg_mutex);
     if (g_pg_configured[dev & 63]) return cudaSuccess;
     e = cudaFuncSetAttribute(pg_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)panel);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(pg_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PG_PANEL_SMEM);
     if (e == cudaSuccess) g_pg_configured[dev & 63] = true;
     return e;
 }
@@ -691,17 +914,38 @@ cudaError_t configure_device(size_t panel) {
 int launch_pg_optimize(const PgLaunch& L, cudaStream_t s) {
     const size_t panel = sizeof(double) * CHOL_NB * CHOL_PS;
     if (configure_device(panel) != cudaSuccess) return -1;
-    const int T = (L.max_D + 1 + 31) / 32;
+    const int T = (std::min(L.max_D, PG_MAX_D) + 1 + 31) / 32;
+    const int Tl = pg_tile_np(L.max_D) / PG_TILE;  // panels of the multi-CTA path, 0 when no member takes it
+    const int chain_ctas = (L.max_D + 1 + 383) / 384;
     int launches = 0;
     pg_setup_kernel<<<L.count, 256, 0, s>>>(L);
     launches++;
     for (int it = 0; it < L.max_iterations; it++) {
         pg_linearize_kernel<<<L.count, 256, 0, s>>>(L);
-        pg_chain_kernel<<<L.count, 384, 0, s>>>(L);
+        pg_chain_kernel<<<dim3(chain_ctas, L.count), 384, 0, s>>>(L);
         pg_border_kernel<<<dim3(T * (T + 1) / 2, L.count), 256, 0, s>>>(L);
+        launches += 3;
+        if (Tl) {
+            pg_tile_kernel<false><<<dim3(Tl * (Tl + 1) / 2, L.count), 256, 0, s>>>(L, -1);
+            launches++;
+            for (int p = 0; p < Tl; p++) {
+                pg_panel_kernel<<<dim3(Tl - p, L.count), 256, PG_PANEL_SMEM, s>>>(L, p);
+                launches++;
+                const int R = Tl - p - 1;
+                if (R > 0) {
+                    pg_tile_kernel<true><<<dim3(R * (R + 1) / 2, L.count), 256, 0, s>>>(L, p);
+                    launches++;
+                }
+            }
+        }
         pg_solve_kernel<<<L.count, 512, panel, s>>>(L);
+        launches++;
+        if (Tl) {
+            pg_solve_large_kernel<<<L.count, 512, 0, s>>>(L);
+            launches++;
+        }
         pg_update_kernel<<<L.count, 256, 0, s>>>(L);
-        launches += 5;
+        launches++;
     }
     pg_finish_kernel<<<L.count, 256, 0, s>>>(L);
     return launches + 1;

@@ -16,10 +16,14 @@
 
 namespace vb {
 
-// Capacity of the border (the dense Schur complement of the loop anchors): 4 columns per free anchor, at most the
-// BA step's dense system size.  The only limit on the number of loop anchors in an optimised range.
+// The border (the dense Schur complement of the loop anchors) has 4 columns per free anchor.  Borders of at most PG_MAX_D
+// columns (the BA step's dense system size) are factored in one CTA in shared memory; larger ones by the multi-CTA
+// path in global memory (tile storage, PG_TILE x PG_TILE tiles).  A graph's anchor capacity (vp_config::max_anchors)
+// is PG_MAX_ANCHORS by default and at most PG_CAP_ANCHORS.
 constexpr int PG_MAX_D = BA_MAX_D;
 constexpr int PG_MAX_ANCHORS = PG_MAX_D / 4;
+constexpr int PG_CAP_ANCHORS = 1024;
+constexpr int PG_TILE = 64;
 // Super-blocks of the chain: 4 consecutive key frames, 16 unknowns.
 constexpr int PG_SB = 4, PG_SBD = 16;
 // Per key frame of the assembled normal equations: diagonal block | 4 blocks to the key frames 1..4 back | loop block.
@@ -68,7 +72,9 @@ PG_LAYOUT_FN PgHdrLayout pg_hdr_layout(int S) {
     return o;
 }
 // bytes of the arena: the header plus every member at capacity
-PG_LAYOUT_FN size_t pg_arena_bytes(int S, int cap_n) { return pg_hdr_layout(S).total + (size_t)S * pg_in_layout(cap_n, PG_MAX_ANCHORS).total; }
+PG_LAYOUT_FN size_t pg_arena_bytes(int S, int cap_n, int cap_anchors = PG_MAX_ANCHORS) {
+    return pg_hdr_layout(S).total + (size_t)S * pg_in_layout(cap_n, cap_anchors).total;
+}
 
 // ---- a member's output block, in doubles: yaw (degrees) and t per key frame of the range (n x 4) | summary.
 //      An even count, so consecutive blocks stay 16-byte aligned.
@@ -86,13 +92,23 @@ struct PgState {
 };
 constexpr int PG_STATE_DOUBLES = (int)((sizeof(PgState) + sizeof(double) - 1) / sizeof(double));
 
-// ---- a member's device workspace at capacity cap_n key frames, in doubles.  W (the chain's border columns
-//      L^-1 B and L^-1 r as column D) has (D + 1) columns at run time; it is sized for PG_MAX_D.
+// ---- a member's device workspace at capacity cap_n key frames and cap_anchors free anchors, in doubles.  W (the chain's
+//      border columns L^-1 B and L^-1 r as column D) has (D + 1) columns at run time; it is sized for the capacity and
+//      also holds the linearisation's edge scratch (180 doubles per key frame).  Sp is the packed border system of the
+//      one-CTA path (D <= PG_MAX_D).  U and yb exist only when the capacity exceeds PG_MAX_D columns: U is the border
+//      system [S z] of the multi-CTA path, its upper triangle in a Np x Np row-major square (Np = D + 1 rounded up to
+//      PG_TILE, z in column D), factored in place except for its diagonal tiles, whose factors go to Ud (one
+//      PG_TILE x PG_TILE tile per panel, stacked); yb is the border part of the step.  These are 16-byte aligned.
 struct PgWorkLayout {
-    size_t state, x, xc, dx, scale, ypr, smeas, blk, g, L, F, W, start, Sp, total;
+    size_t state, x, xc, dx, scale, ypr, smeas, blk, g, L, F, W, start, Sp, U, Ud, yb, total;
 };
-PG_LAYOUT_FN PgWorkLayout pg_work_layout(int cap_n) {
-    const size_t n = (size_t)cap_n, nsb = (size_t)pg_num_sb(cap_n), Dp = PG_MAX_D + 1;
+PG_LAYOUT_FN size_t pg_max_sz(size_t a, size_t b) { return a > b ? a : b; }
+PG_LAYOUT_FN size_t pg_even(size_t d) { return (d + 1) & ~(size_t)1; }
+// columns of the square holding U for a border of D columns (0 on the one-CTA path)
+PG_LAYOUT_FN int pg_tile_np(int D) { return D > PG_MAX_D ? (D + 1 + PG_TILE - 1) / PG_TILE * PG_TILE : 0; }
+PG_LAYOUT_FN PgWorkLayout pg_work_layout(int cap_n, int cap_anchors = PG_MAX_ANCHORS) {
+    const size_t n = (size_t)cap_n, nsb = (size_t)pg_num_sb(cap_n), D = 4 * (size_t)cap_anchors, Dp = D + 1;
+    const size_t Dps = (D < (size_t)PG_MAX_D ? D : (size_t)PG_MAX_D) + 1, Np = (size_t)pg_tile_np((int)D);
     PgWorkLayout o{};
     o.state = 0;
     o.x = (PG_STATE_DOUBLES + 1) & ~1;
@@ -106,9 +122,12 @@ PG_LAYOUT_FN PgWorkLayout pg_work_layout(int cap_n) {
     o.L = o.g + 4 * n;                                    // chain factor: 16 x 16 per super-block
     o.F = o.L + 256 * nsb;                                // chain off-diagonal factor blocks
     o.W = o.F + 256 * nsb;                                // 16 nsb x (D + 1), row-major
-    o.start = o.W + 16 * nsb * Dp;                        // first super-block of each W column (ints, Dp of them)
+    o.start = o.W + pg_max_sz(16 * nsb * Dp, 180 * n);    // first super-block of each W column (ints, Dp of them)
     o.Sp = o.start + (((Dp + 1) / 2 + 1) & ~(size_t)1);   // packed border system (D + 1 rows: S | z)
-    o.total = o.Sp + ((Dp * (Dp + 1) / 2 + 1) & ~(size_t)1);
+    o.U = pg_even(o.Sp + ((Dps * (Dps + 1) / 2 + 1) & ~(size_t)1));
+    o.Ud = o.U + Np * Np;
+    o.yb = o.Ud + Np * PG_TILE;
+    o.total = o.yb + (Np ? pg_even(D) : 0);
     return o;
 }
 

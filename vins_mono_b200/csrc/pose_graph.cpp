@@ -69,6 +69,7 @@ struct vp_graph {
 struct vp_batch {
     vp_config cfg{};
     int S = 0;
+    int cap_anchors = 0;  // free loop anchors an optimised range may hold (vp_config::max_anchors, 0 = PG_MAX_ANCHORS)
     std::string err;
     std::vector<vp_graph*> members;
     char *h_in = nullptr, *d_in = nullptr;
@@ -166,7 +167,7 @@ void release(vp_batch* b) {
 
 int batch_create(const vp_config* cfg, int n, vp_batch** out, std::string* err) {
     *out = nullptr;
-    if (!cfg || n < 1 || cfg->max_keyframes < 2) return VP_ERR_INVALID;
+    if (!cfg || n < 1 || cfg->max_keyframes < 2 || cfg->max_anchors < 0 || cfg->max_anchors > vb::PG_CAP_ANCHORS) return VP_ERR_INVALID;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device < 0 || cfg->device >= ndev) {
         cudaGetLastError();
@@ -176,6 +177,7 @@ int batch_create(const vp_config* cfg, int n, vp_batch** out, std::string* err) 
     vp_batch* b = new vp_batch;
     b->cfg = *cfg;
     b->S = n;
+    b->cap_anchors = cfg->max_anchors ? cfg->max_anchors : vb::PG_MAX_ANCHORS;
     auto fail = [&](cudaError_t e) {
         if (err) *err = cudaGetErrorString(e);
         release(b);
@@ -184,8 +186,8 @@ int batch_create(const vp_config* cfg, int n, vp_batch** out, std::string* err) 
     cudaError_t e = cudaSetDevice(cfg->device);
     if (e != cudaSuccess) return fail(e);
     const int cap = cfg->max_keyframes;
-    b->work_stride = (vb::pg_work_layout(cap).total + 1) & ~(size_t)1;
-    b->in_bytes = vb::pg_arena_bytes(n, cap);
+    b->work_stride = (vb::pg_work_layout(cap, b->cap_anchors).total + 1) & ~(size_t)1;
+    b->in_bytes = vb::pg_arena_bytes(n, cap, b->cap_anchors);
     b->out_doubles = (size_t)n * vb::pg_out_layout(cap).total;
     if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
     if ((e = cudaEventCreate(&b->ev0)) != cudaSuccess || (e = cudaEventCreate(&b->ev1)) != cudaSuccess) return fail(e);
@@ -206,7 +208,7 @@ int batch_create(const vp_config* cfg, int n, vp_batch** out, std::string* err) 
 }
 
 // Packs member g's pending optimisation into the input arena at byte offset `off`.  Fails (changing nothing) when its
-// range has more free loop anchors than the border holds.
+// range has more free loop anchors than the graph's anchor capacity.
 // pr (out) receives the pitch and roll of each key frame of the range (the constants of the solve).  The member itself is
 // not changed.
 int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, std::vector<double>* pr) {
@@ -219,9 +221,9 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, st
     std::sort(anchors.begin(), anchors.end());
     anchors.erase(std::unique(anchors.begin(), anchors.end()), anchors.end());
     const int nb = (int)anchors.size();
-    if (nb > vb::PG_MAX_ANCHORS) {
-        g->err = "vp_optimize: " + std::to_string(nb) + " free loop anchors in the optimised range, at most " +
-                 std::to_string(vb::PG_MAX_ANCHORS);
+    const int cap = g->owner->cap_anchors;
+    if (nb > cap) {
+        g->err = "vp_optimize: " + std::to_string(nb) + " free loop anchors in the optimised range, at most " + std::to_string(cap);
         return VP_ERR_CAPACITY;
     }
     const vb::PgInLayout il = vb::pg_in_layout(n, nb);
@@ -283,7 +285,8 @@ int enqueue(vp_batch* b, size_t in_bytes, size_t out_doubles, int count, int max
     if ((e = cudaSetDevice(b->cfg.device)) != cudaSuccess) return fail("cudaSetDevice", e);
     if ((e = cudaMemcpyAsync(b->d_in, b->h_in, in_bytes, cudaMemcpyHostToDevice, b->stream)) != cudaSuccess) return fail("input copy", e);
     if ((e = cudaEventRecord(b->ev0, b->stream)) != cudaSuccess) return fail("cudaEventRecord", e);
-    vb::PgLaunch L{b->d_in, b->d_work, b->work_stride, b->d_out, b->S, b->cfg.max_keyframes, count, max_n, max_D, PG_MAX_ITERATIONS};
+    vb::PgLaunch L{b->d_in,           b->d_work, b->work_stride, b->d_out, b->S, b->cfg.max_keyframes,
+                   b->cap_anchors, count,     max_n,          max_D,    PG_MAX_ITERATIONS};
     const int launches = vb::launch_pg_optimize(L, b->stream);
     e = cudaGetLastError();
     if (launches < 0 && e == cudaSuccess) e = cudaErrorInvalidConfiguration;

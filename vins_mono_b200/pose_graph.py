@@ -10,7 +10,7 @@ from .tracker import load_library
 
 
 class PoseGraphConfig(C.Structure):
-    _fields_ = [("max_keyframes", C.c_int), ("fast_relocalization", C.c_int), ("device", C.c_int)]
+    _fields_ = [("max_keyframes", C.c_int), ("fast_relocalization", C.c_int), ("device", C.c_int), ("max_anchors", C.c_int)]
 
 
 def _p(a):
@@ -65,16 +65,19 @@ class PoseGraphError(RuntimeError):
 
 
 class PoseGraph:
-    """The reference's PoseGraph with the loop already found: addKeyFrame / updateKeyFrameLoop / optimize4DoF."""
+    """The reference's PoseGraph with the loop already found: addKeyFrame / updateKeyFrameLoop / optimize4DoF.
+    max_anchors: free loop anchors an optimised range may hold (0 = 88, at most 1024); the workspace grows with it."""
 
-    def __init__(self, max_keyframes=2000, fast_relocalization=False, device=0):
+    def __init__(self, max_keyframes=2000, fast_relocalization=False, device=0, max_anchors=0):
         self.lib = load_library()
         _bind(self.lib)
-        self.cfg = PoseGraphConfig(max_keyframes=max_keyframes, fast_relocalization=int(fast_relocalization), device=device)
+        self.cfg = PoseGraphConfig(max_keyframes=max_keyframes, fast_relocalization=int(fast_relocalization), device=device,
+                                   max_anchors=max_anchors)
         h = C.c_void_p()
         rc = self.lib.vp_create(C.byref(self.cfg), C.byref(h))
         if rc != 0:
-            raise RuntimeError(f"vp_create failed with status {rc} (-2 = no CUDA device; this library has no CPU path)")
+            raise RuntimeError(f"vp_create failed with status {rc} (-1 = invalid configuration, -2 = no CUDA device; this library "
+                               "has no CPU path)")
         self.h, self._borrowed = h, False
 
     @classmethod
@@ -155,10 +158,11 @@ class PoseGraph:
 class PoseGraphBatch:
     """n independent pose graphs whose pending optimisations run in one launch chain."""
 
-    def __init__(self, n, max_keyframes=2000, fast_relocalization=False, device=0):
+    def __init__(self, n, max_keyframes=2000, fast_relocalization=False, device=0, max_anchors=0):
         self.lib = load_library()
         _bind(self.lib)
-        self.cfg = PoseGraphConfig(max_keyframes=max_keyframes, fast_relocalization=int(fast_relocalization), device=device)
+        self.cfg = PoseGraphConfig(max_keyframes=max_keyframes, fast_relocalization=int(fast_relocalization), device=device,
+                                   max_anchors=max_anchors)
         h = C.c_void_p()
         rc = self.lib.vp_batch_create(C.byref(self.cfg), int(n), C.byref(h))
         if rc != 0:
