@@ -293,12 +293,15 @@ def loop_frame_matches(seq: Sequence, t_loop: float, ids, n_points: int = 2500, 
 
 
 def track_messages(seq: Sequence, n_pub: int, n_points: int = 2500, max_feats: int = 150, pub_hz: float = 10.0, pixel_sigma: float = 0.3,
-                   start_id: int = 0):
+                   start_id: int = 0, landmarks=None):
     """Feature messages (stamp, ids, xyz_uv_vel[n,7]) made directly from the scene geometry (no images), in the
     spirit of the reference's data_generator (data_generator/src/data_generator.cpp:11-59): random landmarks on
     the room walls, projected through the EuRoC pinhole+radtan model, at most `max_feats` per frame with stable
-    ids, pixel noise sigma `pixel_sigma`.  Back-end tests/benchmarks use this to avoid rendering."""
+    ids, pixel noise sigma `pixel_sigma`.  Back-end tests/benchmarks use this to avoid rendering.  `landmarks` (world points)
+    replaces the random wall points, e.g. with harness/loop_revisit.py's texture corners."""
     pts, rng = scene_landmarks(seq, n_points)
+    if landmarks is not None:
+        pts = np.asarray(landmarks, np.float64)
 
     def project(t):
         p, R, *_ = seq.pose(t)

@@ -13,6 +13,7 @@
 
 #include "cuda_check.h"
 #include "host_math.h"
+#include "pg_host.h"
 #include "pg_kernels.h"
 #include "pg_layout.h"
 
@@ -83,6 +84,7 @@ struct vp_batch {
     std::chrono::steady_clock::time_point t0;
     float ms[2] = {0, 0};
     int launches = 0;
+    vb::LvState* lv = nullptr;  // loop verification (loop_verify.cpp), once enabled
 };
 
 namespace {
@@ -152,6 +154,7 @@ int collect(vp_graph* g) {
 }
 
 void release(vp_batch* b) {
+    vb::lv_release(b->lv);
     if (b->stream) cudaStreamSynchronize(b->stream);
     cudaFreeHost(b->h_in);
     cudaFreeHost(b->h_out);
@@ -379,6 +382,21 @@ void store_pose(const KeyFrame& kf, double* P3, double* Q4) {
 }
 
 }  // namespace
+
+namespace vb {
+LvState** pg_loop_state(vp_batch* b) { return &b->lv; }
+vp_batch* pg_owner(vp_graph* g, int* member, bool* standalone) {
+    *member = g->member;
+    *standalone = g->standalone;
+    return g->owner;
+}
+int pg_capacity(const vp_batch* b, int* device) {
+    *device = b->cfg.device;
+    return b->cfg.max_keyframes;
+}
+std::string* pg_error(vp_graph* g) { return &g->err; }
+std::string* pg_batch_error(vp_batch* b) { return &b->err; }
+}  // namespace vb
 
 extern "C" {
 

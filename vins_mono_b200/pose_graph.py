@@ -213,3 +213,169 @@ def debug_four_dof_error(params8, meas6, weighted=False, robust=False):
     if rc != 0:
         raise RuntimeError(f"vp_debug_four_dof_error failed with status {rc}")
     return out[:4], out[4:36].reshape(4, 8), out[36]
+
+
+# ---- loop verification (include/vinsb200/loop_verify.h)
+
+class LoopConfig(C.Structure):
+    _fields_ = [("rows", C.c_int), ("cols", C.c_int), ("intrinsics", C.c_double * 8), ("ric9", C.c_double * 9), ("tic3", C.c_double * 3),
+                ("brief_pattern", C.c_void_p), ("max_window", C.c_int), ("max_corners", C.c_int)]
+
+
+class LoopResult(C.Structure):
+    _fields_ = [("accepted", C.c_int), ("n_matches", C.c_int), ("n_inliers", C.c_int), ("n_points", C.c_int),
+                ("loop_info", C.c_double * 8), ("old_R9", C.c_double * 9), ("old_T3", C.c_double * 3)]
+
+
+def _bind_loop(lib):
+    V = C.c_void_p
+    lib.vp_loop_enable.argtypes = [V, C.POINTER(LoopConfig)]
+    lib.vp_batch_loop_enable.argtypes = [V, C.POINTER(LoopConfig)]
+    lib.vp_attach_keyframe.argtypes = [V, C.c_int, V, V, V, C.c_size_t, C.c_int, V, V, V, V, C.POINTER(C.c_int)]
+    lib.vp_find_connection.argtypes = [V, C.c_int, C.c_int, C.POINTER(LoopResult), C.c_int, V]
+    lib.vp_batch_find_connection.argtypes = [V, V, V, V, C.c_int, V, V]
+    lib.vp_loop_last_timing.argtypes = [V, V]
+    lib.vp_batch_loop_last_timing.argtypes = [V, V]
+    lib.vp_debug_brief_blur.argtypes = [V, C.c_int, C.c_int, V]
+    lib.vp_debug_fast.argtypes = [V, C.c_int, C.c_int, C.c_int, V]
+    lib.vp_debug_brief.argtypes = [V, C.c_int, C.c_int, V, C.c_int, V, V]
+    lib.vp_debug_match.argtypes = [C.c_int, V, C.c_int, V, V]
+    lib.vp_debug_pnp.argtypes = [C.c_int, V, V, V, C.POINTER(C.c_int), V]
+
+
+def loop_config(rows, cols, intrinsics, ric, tic, pattern, max_window=256, max_corners=4096):
+    pat = np.ascontiguousarray(pattern, np.int32).reshape(256, 4)
+    cfg = LoopConfig(rows=rows, cols=cols, max_window=max_window, max_corners=max_corners)
+    cfg.intrinsics[:] = [float(v) for v in intrinsics]
+    cfg.ric9[:] = [float(v) for v in np.asarray(ric, np.float64).reshape(9)]
+    cfg.tic3[:] = [float(v) for v in np.asarray(tic, np.float64).reshape(3)]
+    cfg.brief_pattern = pat.ctypes.data
+    cfg._pattern = pat  # kept alive until the enable call has copied it
+    return cfg
+
+
+def _result(r, lst):
+    return dict(accepted=bool(r.accepted), n_matches=r.n_matches, n_inliers=r.n_inliers, loop_info=np.array(r.loop_info[:]),
+                old_R=np.array(r.old_R9[:]).reshape(3, 3), old_T=np.array(r.old_T3[:]), points=lst[:r.n_points].copy())
+
+
+def _enable_loop(self, cfg):
+    _bind_loop(self.lib)
+    self._loop_cap = cfg.max_window
+    self._check(self.lib.vp_loop_enable(self.h, C.byref(cfg)))
+
+
+def _attach_keyframe(self, index, vio_P, vio_Q_wxyz, image, point_3d, point_uv, point_norm, point_id):
+    """KeyFrame's constructor: descriptors of the window points and of the FAST corners.  Returns the corner count."""
+    img = np.ascontiguousarray(image, np.uint8)
+    p3, uv = np.ascontiguousarray(point_3d, np.float32).reshape(-1, 3), np.ascontiguousarray(point_uv, np.float32).reshape(-1, 2)
+    nm, ids = np.ascontiguousarray(point_norm, np.float32).reshape(-1, 2), np.ascontiguousarray(point_id, np.float64).reshape(-1)
+    nc = C.c_int()
+    self._check(self.lib.vp_attach_keyframe(self.h, int(index), _p(_d(vio_P)), _p(_d(vio_Q_wxyz)), _p(img), img.strides[0], len(p3),
+                                            _p(p3), _p(uv), _p(nm), _p(ids), C.byref(nc)))
+    return nc.value
+
+
+def _find_connection(self, cur, old):
+    """findConnection: dict(accepted, n_matches, n_inliers, loop_info 8, old_R, old_T, points = inliers' (x, y, id))."""
+    r, lst = LoopResult(), np.zeros((self._loop_cap, 3))
+    self._check(self.lib.vp_find_connection(self.h, int(cur), int(old), C.byref(r), self._loop_cap, _p(lst)))
+    return _result(r, lst)
+
+
+def _loop_timing(self):
+    ms = np.zeros(6, np.float32)
+    self._check(self.lib.vp_loop_last_timing(self.h, _p(ms)))
+    return ms
+
+
+PoseGraph.enable_loop = _enable_loop
+PoseGraph.attach_keyframe = _attach_keyframe
+PoseGraph.find_connection = _find_connection
+PoseGraph.loop_timing = _loop_timing
+
+
+def _batch_enable_loop(self, cfg):
+    _bind_loop(self.lib)
+    self._loop_cap = cfg.max_window
+    for m in self.members:
+        m._loop_cap = cfg.max_window
+    rc = self.lib.vp_batch_loop_enable(self.h, C.byref(cfg))
+    if rc < 0:
+        raise PoseGraphError(rc, self.lib.vp_batch_last_error(self.h).decode())
+
+
+def _batch_find_connection(self, cur, old):
+    """One launch chain for every member k with cur[k] >= 0; returns a list (None for skipped members)."""
+    res = (LoopResult * self.n)()
+    lst = np.zeros((self.n, self._loop_cap, 3))
+    st = np.zeros(self.n, np.int32)
+    c, o = np.ascontiguousarray(cur, np.int32), np.ascontiguousarray(old, np.int32)
+    rc = self.lib.vp_batch_find_connection(self.h, _p(c), _p(o), res, self._loop_cap, _p(lst), _p(st))
+    if rc < 0:
+        raise PoseGraphError(rc, self.lib.vp_batch_last_error(self.h).decode())
+    return [_result(res[k], lst[k]) if st[k] == 1 else None for k in range(self.n)]
+
+
+def _batch_loop_timing(self):
+    ms = np.zeros(6, np.float32)
+    self.lib.vp_batch_loop_last_timing(self.h, _p(ms))
+    return ms
+
+
+PoseGraphBatch.enable_loop = _batch_enable_loop
+PoseGraphBatch.find_connection = _batch_find_connection
+PoseGraphBatch.loop_timing = _batch_loop_timing
+
+
+def _lib():
+    lib = load_library()
+    _bind_loop(lib)
+    return lib
+
+
+def debug_brief_blur(image):
+    img = np.ascontiguousarray(image, np.uint8)
+    out = np.zeros_like(img)
+    rc = _lib().vp_debug_brief_blur(_p(img), img.shape[0], img.shape[1], _p(out))
+    if rc:
+        raise RuntimeError(f"vp_debug_brief_blur failed with status {rc}")
+    return out
+
+
+def debug_fast(image, cap=65536):
+    img = np.ascontiguousarray(image, np.uint8)
+    xy = np.zeros((cap, 2), np.float32)
+    n = _lib().vp_debug_fast(_p(img), img.shape[0], img.shape[1], cap, _p(xy))
+    if n < 0:
+        raise RuntimeError(f"vp_debug_fast failed with status {n}")
+    return xy[:n].astype(np.int32)
+
+
+def debug_brief(image, pattern, uv):
+    img = np.ascontiguousarray(image, np.uint8)
+    pat = np.ascontiguousarray(pattern, np.int32)
+    pts = np.ascontiguousarray(uv, np.float32).reshape(-1, 2)
+    desc = np.zeros((len(pts), 4), np.uint64)
+    rc = _lib().vp_debug_brief(_p(img), img.shape[0], img.shape[1], _p(pat), len(pts), _p(pts), _p(desc))
+    if rc:
+        raise RuntimeError(f"vp_debug_brief failed with status {rc}")
+    return desc
+
+
+def debug_match(desc_a, desc_b):
+    a, b = np.ascontiguousarray(desc_a, np.uint64), np.ascontiguousarray(desc_b, np.uint64)
+    idx = np.zeros(len(a), np.int32)
+    rc = _lib().vp_debug_match(len(a), _p(a), len(b), _p(b) if len(b) else None, _p(idx))
+    if rc:
+        raise RuntimeError(f"vp_debug_match failed with status {rc}")
+    return idx
+
+
+def debug_pnp(point_3d, norm):
+    p3, nm = np.ascontiguousarray(point_3d, np.float32).reshape(-1, 3), np.ascontiguousarray(norm, np.float32).reshape(-1, 2)
+    Rt, n_in, mask = np.zeros(12), C.c_int(), np.zeros(len(p3), np.uint8)
+    rc = _lib().vp_debug_pnp(len(p3), _p(p3), _p(nm), _p(Rt), C.byref(n_in), _p(mask))
+    if rc:
+        raise RuntimeError(f"vp_debug_pnp failed with status {rc}")
+    return Rt[:9].reshape(3, 3), Rt[9:], n_in.value, mask.astype(bool)
