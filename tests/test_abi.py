@@ -17,7 +17,7 @@ def declared_functions():
     for f in sorted(os.listdir(inc)):
         src = open(os.path.join(inc, f)).read()
         src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-        names += re.findall(r"\b(v[ter]_[a-z0-9_]+)\s*\(", src)
+        names += re.findall(r"\b(v[terp]_[a-z0-9_]+)\s*\(", src)
     return sorted(set(names))
 
 

@@ -15,8 +15,10 @@
 // the FP64 pipe is far from saturated, so no tensor-core path is used (see DESIGN.md).
 #include "ba_kernels.h"
 #include "ba_layout.h"
+#include "cuda_check.h"
 
 #include <algorithm>
+#include <map>
 #include <mutex>
 #include <cfloat>
 
@@ -1322,20 +1324,19 @@ namespace vb {
 
 namespace {
 
-// Per-device launch configuration: function attributes (the opt-in to > 48 KB dynamic shared memory) belong to the
-// device the calling thread has current, and handles may live on different GPUs of one process.
+// What the launches query of the current device: its opt-in shared-memory limit and the kernels' static shared sizes
+// (handles may live on different GPUs of one process).
 struct DeviceCfg {
     bool init = false;
     int smem_limit = 0, step_static = 0, marg_static = 0;
-    int step_configured = 0, marg_configured = 0;
 };
 std::mutex g_cfg_mutex;
-DeviceCfg g_cfg[64];
+std::map<int, DeviceCfg> g_cfg;
 
 DeviceCfg& device_cfg_locked() {  // caller holds g_cfg_mutex
     int dev = 0;
     cudaGetDevice(&dev);
-    DeviceCfg& c = g_cfg[dev & 63];
+    DeviceCfg& c = g_cfg[dev];
     if (!c.init) {
         cudaDeviceGetAttribute(&c.smem_limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
         cudaFuncAttributes fa{};
@@ -1388,12 +1389,7 @@ void launch_reduce(const BaSeq* seqs, const BatchShape& sh, cudaStream_t s) {
 // Dynamic shared memory of marg_solve_kernel at the batch's maxima, with the kernel's opt-in on this device raised to it
 size_t prepare_marg_solve(const BatchShape& sh) {
     const size_t smem = marg_solve_smem_bytes(sh.max_md, sh.max_n, sh.w_in_global != 0);
-    std::lock_guard<std::mutex> lock(g_cfg_mutex);
-    DeviceCfg& c = device_cfg_locked();
-    if ((int)smem > c.marg_configured) {
-        cudaFuncSetAttribute(marg_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        c.marg_configured = (int)smem;
-    }
+    raise_dynamic_smem((const void*)marg_solve_kernel, (int)smem);
     return smem;
 }
 
@@ -1410,17 +1406,13 @@ void launch_ba_solve(BaSeq* seqs, const BatchShape& sh, cudaStream_t s, int* lau
     const size_t panel_bytes = sizeof(double) * CHOL_NB * CHOL_PS;
     const size_t chol_bytes = sizeof(double) * (size_t)(sh.D + 1) * (sh.D + 2) / 2 + panel_bytes;
     int use_smem;
-    size_t step_dyn;
     {
         std::lock_guard<std::mutex> lock(g_cfg_mutex);
         DeviceCfg& c = device_cfg_locked();
         use_smem = chol_bytes + (size_t)c.step_static + 256 <= (size_t)c.smem_limit ? 1 : 0;
-        step_dyn = use_smem ? chol_bytes : panel_bytes;
-        if ((int)step_dyn > c.step_configured) {
-            cudaFuncSetAttribute(ba_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_dyn);
-            c.step_configured = (int)step_dyn;
-        }
     }
+    const size_t step_dyn = use_smem ? chol_bytes : panel_bytes;
+    raise_dynamic_smem((const void*)ba_step_kernel, (int)step_dyn);
     int n = 0;
     prof->begin(s);
     launch_eval(seqs, sh, eval_grid, 1, s);

@@ -20,6 +20,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -62,20 +63,6 @@ struct SeedRow {
 
 struct PriorBlock {
     int type, index, off, size;  // type 0 pose, 1 speed-bias, 2 ex pose, 3 td; size = local size
-};
-
-template <class T>
-struct DeviceBuf {
-    T* p = nullptr;
-    size_t n = 0;
-    cudaError_t alloc(size_t count) {
-        n = count;
-        return cudaMalloc(&p, sizeof(T) * std::max<size_t>(count, 1));
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-    }
 };
 
 enum FrameStage { STAGE_DONE = 0, STAGE_INIT_SOLVE = 1, STAGE_RUN_SOLVE = 2 };
@@ -161,12 +148,12 @@ struct ve_estimator {
     int marg_n = 0;
     // ---- persistent device memory of this member
     int Lmax = 0, Mmax = 0, D = 0, nmax = 0;
-    DeviceBuf<vb::PreInt> d_preint;
-    DeviceBuf<double> d_states1;     // x[1] (x[0] lives in the frame's input block)
-    DeviceBuf<double> d_acc[2];      // Hpp | gp | Hpl | Hll | gl | cost
-    DeviceBuf<double> d_S, d_Spk, d_Hfull, d_gred, d_vec, d_work;
-    DeviceBuf<double> d_prior[2];    // A | g0 | c0 | x0
-    DeviceBuf<double> d_marg;        // Am | bm | Araw | graw | Wglobal
+    vb::DeviceArray<vb::PreInt> d_preint;
+    vb::DeviceArray<double> d_states1;     // x[1] (x[0] lives in the frame's input block)
+    vb::DeviceArray<double> d_acc[2];      // Hpp | gp | Hpl | Hll | gl | cost
+    vb::DeviceArray<double> d_S, d_Spk, d_Hfull, d_gred, d_vec, d_work;
+    vb::DeviceArray<double> d_prior[2];    // A | g0 | c0 | x0
+    vb::DeviceArray<double> d_marg;        // Am | bm | Araw | graw | Wglobal
 };
 
 struct ve_batch {
@@ -180,8 +167,8 @@ struct ve_batch {
     // single-CTA-per-member solvers of one group leave most SMs to the wide kernels of another).
     struct Group {
         int first = 0, count = 0;
-        cudaStream_t stream = nullptr, copy_stream = nullptr;
-        cudaEvent_t ev[8] = {};  // 0 frame start, 1 after pre-integration, 2 after the solve + re-anchoring, 3 marginalisation done,
+        vb::Stream stream, copy_stream;
+        vb::Event ev[8];  // 0 frame start, 1 after pre-integration, 2 after the solve + re-anchoring, 3 marginalisation done,
                                  // 4 results on the host, 5 marginalisation start
         size_t in_base = 0, in_cap = 0;    // bytes, slice of the input arena
         size_t out_base = 0, out_cap = 0;  // doubles, slice of the output arena
@@ -189,16 +176,16 @@ struct ve_batch {
         bool waits_results = false, has_marg = false;
     };
     int G = 1;
-    Group* groups = nullptr;
+    std::unique_ptr<Group[]> groups;
     int members_per_group = 1;
-    vb::BaSeq* h_seq = nullptr;  // pinned mirror of d_seq
-    vb::BaSeq* d_seq = nullptr;
-    unsigned char* h_in = nullptr;  // pinned: packed per-member input blocks of the frame
-    unsigned char* d_in = nullptr;
-    double* h_out = nullptr;        // pinned: per-member output blocks
-    double* d_out = nullptr;
+    vb::PinnedArray<vb::BaSeq> h_seq;  // mirror of d_seq
+    vb::DeviceArray<vb::BaSeq> d_seq;
+    vb::PinnedArray<unsigned char> h_in;  // packed per-member input blocks of the frame
+    vb::DeviceArray<unsigned char> d_in;
+    vb::PinnedArray<double> h_out;        // per-member output blocks
+    vb::DeviceArray<double> d_out;
     vb::KernelProfile prof;
-    vb::HostPool* pool = nullptr;
+    std::unique_ptr<vb::HostPool> pool;
     float last_ms[4] = {0, 0, 0, 0};
     int last_launches = 0;
     bool marg_timing_valid = false;
@@ -818,7 +805,7 @@ int stage_frame(ve_estimator* e, bool solve) {
     q.jobs = din.jobs;
     q.samples = din.samples;
     q.noise[0] = e->cfg.acc_n; q.noise[1] = e->cfg.gyr_n; q.noise[2] = e->cfg.acc_w; q.noise[3] = e->cfg.gyr_w;
-    q.p.preint = e->d_preint.p;
+    q.p.preint = e->d_preint;
     e->jobs.clear();
     e->job_samples.clear();
     if (!solve) return VE_OK;
@@ -884,13 +871,13 @@ int stage_frame(ve_estimator* e, bool solve) {
     d.half_row = e->cfg.row / 2;
     d.G[0] = 0; d.G[1] = 0; d.G[2] = e->cfg.g_norm;
     p.x[0] = vb::states_view(din.states, F, L);
-    p.x[1] = vb::states_view(e->d_states1.p, F, L);
+    p.x[1] = vb::states_view(e->d_states1, F, L);
     const bool wide = d.est_ex || d.est_td;
     d.oj = wide ? vb::OJ_FULL : vb::OJ_BASE;
     d.lw = wide ? vb::LW_FULL : vb::LW_BASE;
     const vb::BaAccLayout al = vb::ba_acc_layout(W, e->Lmax, e->Mmax, e->D);
     for (int k = 0; k < 2; k++) {  // sized for the widest records; the kernels index with dims.oj / dims.lw
-        double* a = e->d_acc[k].p;
+        double* a = e->d_acc[k];
         p.acc[k] = vb::BaAccum{a + al.obsJ, a + al.lmW, a + al.imuJ, a + al.gpr, a + al.gp, a + al.cost};
     }
     p.lm_anchor = din.lm_anchor;
@@ -922,22 +909,22 @@ int stage_frame(ve_estimator* e, bool solve) {
         pr.type = dq->prior_type;  // addresses inside the device copy of this descriptor
         pr.index = dq->prior_index;
         pr.off = dq->prior_off;
-        const double* a = e->d_prior[e->prior_buf].p;
+        const double* a = e->d_prior[e->prior_buf];
         pr.A = a + pl.A;
         pr.g0 = a + pl.g0;
         pr.c0 = a + pl.c0;
         pr.x0 = a + pl.x0;
     }
-    p.S = e->d_S.p;
-    p.Spk = e->d_Spk.p;
-    p.Hfull = e->d_Hfull.p;
-    p.gred = e->d_gred.p;
+    p.S = e->d_S;
+    p.Spk = e->d_Spk;
+    p.Hfull = e->d_Hfull;
+    p.gred = e->d_gred;
     const vb::BaVecLayout vl = vb::ba_vec_layout(e->D, e->Lmax);
-    p.scale = e->d_vec.p + vl.scale;
-    p.diag = e->d_vec.p + vl.diag;
-    p.grad = e->d_vec.p + vl.grad;
-    p.gn = e->d_vec.p + vl.gn;
-    p.work = e->d_work.p;
+    p.scale = e->d_vec + vl.scale;
+    p.diag = e->d_vec + vl.diag;
+    p.grad = e->d_vec + vl.grad;
+    p.gn = e->d_vec + vl.gn;
+    p.work = e->d_work;
     p.st = &dq->st;
     vb::SolverState& st = q.st;
     std::memset(&st, 0, sizeof(st));
@@ -978,22 +965,22 @@ int stage_frame(ve_estimator* e, bool solve) {
         mp.lms = din.marg_lms;
         mp.col_lm = din.marg_col_lm;
         const vb::BaMargLayout ml = vb::ba_marg_layout(e->nmax, e->Lmax);
-        mp.Am = e->d_marg.p + ml.Am;
-        mp.bm = e->d_marg.p + ml.bm;
-        mp.Araw = e->d_marg.p + ml.Araw;
-        mp.graw = e->d_marg.p + ml.graw;
-        mp.Wglobal = e->d_marg.p + ml.Wglobal;
+        mp.Am = e->d_marg + ml.Am;
+        mp.bm = e->d_marg + ml.bm;
+        mp.Araw = e->d_marg + ml.Araw;
+        mp.graw = e->d_marg + ml.graw;
+        mp.Wglobal = e->d_marg + ml.Wglobal;
         mp.w_in_global = b->w_in_global;  // fixed at batch creation
         const int nb = e->prior_buf ^ 1;
-        mp.Aout = e->d_prior[nb].p + pl.A;  // written with leading dimension n (dense n x n at the front of the buffer)
-        mp.gout = e->d_prior[nb].p + pl.g0;
-        mp.cout = e->d_prior[nb].p + pl.c0;
+        mp.Aout = e->d_prior[nb] + pl.A;  // written with leading dimension n (dense n x n at the front of the buffer)
+        mp.gout = e->d_prior[nb] + pl.g0;
+        mp.cout = e->d_prior[nb] + pl.c0;
         fp.n_kept = (int)mh.kept.size();
         for (int k = 0; k < fp.n_kept; k++) {
             fp.kept_type[k] = mh.kept[k].type;
             fp.kept_index[k] = mh.kept[k].index;
         }
-        fp.x0_out = e->d_prior[nb].p + pl.x0;
+        fp.x0_out = e->d_prior[nb] + pl.x0;
         q.mp = mp;
         q.do_marg = 1;
         e->fr_marg = true;
@@ -1298,15 +1285,6 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
     return rc;
 }
 
-void destroy_member(ve_estimator* e) {
-    if (!e) return;
-    e->d_preint.release(); e->d_states1.release();
-    for (int k = 0; k < 2; k++) { e->d_acc[k].release(); e->d_prior[k].release(); }
-    e->d_S.release(); e->d_Spk.release(); e->d_Hfull.release(); e->d_gred.release(); e->d_vec.release();
-    e->d_work.release(); e->d_marg.release();
-    delete e;
-}
-
 int config_valid(const ve_config* cfg) {
     if (cfg->window_size < 3 || cfg->window_size + 1 > vb::BA_MAX_FRAMES || cfg->window_size + 1 > vb::BA_MAX_OBS_PER_LM ||
         cfg->max_features < 8 || cfg->num_iterations < 1 || cfg->estimate_extrinsic > 2 || cfg->estimate_extrinsic < 0)
@@ -1317,8 +1295,9 @@ int config_valid(const ve_config* cfg) {
     return 1;
 }
 
-ve_estimator* create_member(ve_batch* b, int k) {
-    ve_estimator* e = new ve_estimator();
+// Creates member k and appends it to the batch.
+int create_member(ve_batch* b, int k) {
+    std::unique_ptr<ve_estimator> e(new ve_estimator());
     e->cfg = b->cfg;
     e->batch = b;
     e->member = k;
@@ -1336,22 +1315,23 @@ ve_estimator* create_member(ve_batch* b, int k) {
     e->Mmax = b->cfg.max_features * (W + 1);  // + one relocalisation match per landmark
     e->D = 15 * F + 6 + 1 + 6;               // ex, td and a relocalisation pose on top of the window
     e->nmax = 6 * F + 9 * 2 + 6 + 1;
-    clear_state(e);
-    set_parameter(e);
-    bool ok = e->d_preint.alloc(F) == cudaSuccess && e->d_states1.alloc(vb::ba_states_layout(F, e->Lmax).total) == cudaSuccess;
-    for (int k2 = 0; k2 < 2 && ok; k2++)
-        ok = e->d_acc[k2].alloc(vb::ba_acc_layout(W, e->Lmax, e->Mmax, e->D).total) == cudaSuccess &&
-             e->d_prior[k2].alloc(vb::ba_prior_layout(e->nmax).total) == cudaSuccess;
-    ok = ok && e->d_S.alloc((size_t)e->D * e->D) == cudaSuccess && e->d_Spk.alloc(vb::ba_spk_doubles(e->D)) == cudaSuccess &&
-         e->d_Hfull.alloc((size_t)e->D * e->D) == cudaSuccess && e->d_gred.alloc(e->D) == cudaSuccess &&
-         e->d_vec.alloc(vb::ba_vec_layout(e->D, e->Lmax).total) == cudaSuccess &&
-         e->d_work.alloc(vb::ba_work_layout(e->D, e->Lmax).total) == cudaSuccess &&
-         e->d_marg.alloc(vb::ba_marg_layout(e->nmax, e->Lmax).total) == cudaSuccess;
-    if (!ok) {
-        destroy_member(e);
-        return nullptr;
+    clear_state(e.get());
+    set_parameter(e.get());
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_preint.alloc(F));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_states1.alloc(vb::ba_states_layout(F, e->Lmax).total));
+    for (int k2 = 0; k2 < 2; k2++) {
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_acc[k2].alloc(vb::ba_acc_layout(W, e->Lmax, e->Mmax, e->D).total));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_prior[k2].alloc(vb::ba_prior_layout(e->nmax).total));
     }
-    return e;
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_S.alloc((size_t)e->D * e->D));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_Spk.alloc(vb::ba_spk_doubles(e->D)));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_Hfull.alloc((size_t)e->D * e->D));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_gred.alloc(e->D));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_vec.alloc(vb::ba_vec_layout(e->D, e->Lmax).total));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_work.alloc(vb::ba_work_layout(e->D, e->Lmax).total));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_marg.alloc(vb::ba_marg_layout(e->nmax, e->Lmax).total));
+    b->members.push_back(e.release());
+    return VE_OK;
 }
 
 }  // namespace
@@ -1362,16 +1342,11 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
     if (!cfg || !out || n < 1 || n > 4096) return VE_ERR_INVALID;
     *out = nullptr;
     if (!config_valid(cfg)) return VE_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev) return VE_ERR_NO_DEVICE;
-    ve_batch* b = new ve_batch();
+    if (!vb::device_available(cfg->device)) return VE_ERR_NO_DEVICE;
+    std::unique_ptr<ve_batch, void (*)(ve_batch*)> b(new ve_batch(), ve_batch_destroy);
     b->cfg = *cfg;
     b->S = n;
-    auto fail = [&](int code) {
-        ve_batch_destroy(b);
-        return code;
-    };
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaSetDevice(cfg->device));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaSetDevice(cfg->device));
     // launch groups: VINSB200_BATCH_GROUPS overrides the default (two groups for batches of 32 members and more)
     // measured on an H100 SXM (400 W limit), 64 members, two alternating runs each: 1 group 6.50 / 6.55 k, 2 groups
     // 6.78 / 5.91 k, 3 groups 6.71 / 6.37 k, 4 groups 6.89 / 6.69 k frames/s, i.e. within the run-to-run spread
@@ -1381,19 +1356,18 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
     b->G = G;
     b->members_per_group = (n + G - 1) / G;
     b->G = G = (n + b->members_per_group - 1) / b->members_per_group;
-    b->groups = new ve_batch::Group[G];
+    b->groups.reset(new ve_batch::Group[G]);
     for (int g = 0; g < G; g++) {
         ve_batch::Group& grp = b->groups[g];
         grp.first = g * b->members_per_group;
         grp.count = std::min(b->members_per_group, n - grp.first);
-        VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaStreamCreateWithFlags(&grp.stream, cudaStreamNonBlocking));
-        VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaStreamCreateWithFlags(&grp.copy_stream, cudaStreamNonBlocking));
-        for (auto& ev : grp.ev) VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaEventCreate(&ev));
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, grp.stream.create());
+        VB_CUDA_CHECK(b, VE_ERR_CUDA, grp.copy_stream.create());
+        for (auto& ev : grp.ev) VB_CUDA_CHECK(b, VE_ERR_CUDA, ev.create());
     }
     for (int k = 0; k < n; k++) {
-        ve_estimator* e = create_member(b, k);
-        if (!e) return fail(VE_ERR_CUDA);
-        b->members.push_back(e);
+        const int rc = create_member(b.get(), k);
+        if (rc) return rc;
     }
     const ve_estimator* e0 = b->members[0];
     const int W = cfg->window_size, F = W + 1;
@@ -1412,16 +1386,16 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
         grp.out_cap = vb::ba_out_reserve(F, e0->Lmax, true) * at_cap + vb::ba_out_reserve(F, 256, true) * (size_t)grp.count;
         out_total += grp.out_cap;
     }
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_seq, sizeof(vb::BaSeq) * n));
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_seq, sizeof(vb::BaSeq) * n, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->d_seq.alloc(n));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->h_seq.alloc(n));
     std::memset(b->h_seq, 0, sizeof(vb::BaSeq) * n);
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_in, in_total));
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_in, in_total, cudaHostAllocDefault));
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaMalloc(&b->d_out, sizeof(double) * out_total));
-    VB_CUDA_CHECK(b, fail(VE_ERR_CUDA), cudaHostAlloc(&b->h_out, sizeof(double) * out_total, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->d_in.alloc(in_total));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->h_in.alloc(in_total));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->d_out.alloc(out_total));
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, b->h_out.alloc(out_total));
     b->w_in_global = vb::marg_w_in_global(vb::BA_MARG_MAX_DENSE, e0->nmax);
-    b->pool = new vb::HostPool(vb::HostPool::default_workers(n));
-    *out = b;
+    b->pool.reset(new vb::HostPool(vb::HostPool::default_workers(n)));
+    *out = b.release();
     return VE_OK;
 }
 
@@ -1432,17 +1406,8 @@ void ve_batch_destroy(ve_batch* b) {
         if (b->groups[g].stream) cudaStreamSynchronize(b->groups[g].stream);
         if (b->groups[g].copy_stream) cudaStreamSynchronize(b->groups[g].copy_stream);
     }
-    delete b->pool;
-    for (auto* e : b->members) destroy_member(e);
-    cudaFree(b->d_seq); cudaFree(b->d_in); cudaFree(b->d_out);
-    cudaFreeHost(b->h_seq); cudaFreeHost(b->h_in); cudaFreeHost(b->h_out);
-    for (int g = 0; b->groups && g < b->G; g++) {
-        for (auto& ev : b->groups[g].ev)
-            if (ev) cudaEventDestroy(ev);
-        if (b->groups[g].stream) cudaStreamDestroy(b->groups[g].stream);
-        if (b->groups[g].copy_stream) cudaStreamDestroy(b->groups[g].copy_stream);
-    }
-    delete[] b->groups;
+    b->pool.reset();
+    for (auto* e : b->members) delete e;
     delete b;
 }
 
@@ -1485,6 +1450,7 @@ int ve_batch_last_timing(const ve_batch* cb, float* ms4, int* launches) {
 
 int ve_batch_set_profile(ve_batch* b, int on) {
     if (!b) return VE_ERR_INVALID;
+    VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaSetDevice(b->cfg.device));
     b->prof.enable(on != 0);
     return VE_OK;
 }
@@ -1771,32 +1737,25 @@ int ve_last_timing(const ve_estimator* e, float* ms4, int* launches) { return e 
 int ve_debug_projection_factor(const double* params23, const double* data12, int use_td, double focal_length, double tr, double row,
                                int robust, double* out43) {
     if (!params23 || !data12 || !out43) return VE_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return VE_ERR_NO_DEVICE;
-    double* d = nullptr;
-    if (cudaMalloc(&d, sizeof(double) * (23 + 12 + 43)) != cudaSuccess) return VE_ERR_CUDA;
+    if (!vb::device_available(0)) return VE_ERR_NO_DEVICE;
+    vb::DeviceArray<double> d;
+    if (d.alloc(23 + 12 + 43) != cudaSuccess) return VE_ERR_CUDA;
     vb::BaDims dm{};
     dm.est_td = use_td ? 1 : 0;
     dm.sqrt_info_vis = focal_length / 1.5;
     dm.tr_over_row = tr / row;
     dm.half_row = row / 2;
-    int rc = VE_OK;
     if (cudaMemcpy(d, params23, sizeof(double) * 23, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(d + 23, data12, sizeof(double) * 12, cudaMemcpyHostToDevice) != cudaSuccess)
-        rc = VE_ERR_CUDA;
-    if (rc == VE_OK) {
-        vb::launch_debug_visual(dm, d, d + 23, robust, d + 35, nullptr);
-        if (cudaMemcpy(out43, d + 35, sizeof(double) * 43, cudaMemcpyDeviceToHost) != cudaSuccess) rc = VE_ERR_CUDA;
-    }
-    cudaFree(d);
-    return rc;
+        return VE_ERR_CUDA;
+    vb::launch_debug_visual(dm, d, d + 23, robust, d + 35, nullptr);
+    return cudaMemcpy(out43, d + 35, sizeof(double) * 43, cudaMemcpyDeviceToHost) == cudaSuccess ? VE_OK : VE_ERR_CUDA;
 }
 
 int ve_debug_imu_factor(const double* noise4, double g_norm, const double* ba, const double* bg, int n, const double* dt,
                         const double* acc, const double* gyr, const double* params32, double* out_preint, double* out_factor) {
     if (!noise4 || !ba || !bg || n < 1 || !dt || !acc || !gyr) return VE_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return VE_ERR_NO_DEVICE;
+    if (!vb::device_available(0)) return VE_ERR_NO_DEVICE;
     // sample 0 seeds the IntegrationBase (acc_0 / gyr_0), samples 1..n-1 are pushed with dt[k]
     vb::BaSeq q{};
     vb::PreintJob jobs[2]{};
@@ -1818,12 +1777,12 @@ int ve_debug_imu_factor(const double* noise4, double g_norm, const double* ba, c
             r[4 + c] = gyr[3 * k + c];
         }
     }
-    unsigned char* d = nullptr;
+    vb::DeviceArray<unsigned char> d;
     using vb::ba_align16;
     const size_t o_seq = 0, o_jobs = ba_align16(sizeof(vb::BaSeq)), o_rec = o_jobs + ba_align16(sizeof(jobs)),
                  o_pre = o_rec + ba_align16(rec.size() * sizeof(double)), o_prm = o_pre + ba_align16(sizeof(vb::PreInt)),
                  o_out = o_prm + ba_align16(32 * sizeof(double)), total = o_out + ba_align16(465 * sizeof(double));
-    if (cudaMalloc(&d, total) != cudaSuccess) return VE_ERR_CUDA;
+    if (d.alloc(total) != cudaSuccess) return VE_ERR_CUDA;
     q.n_jobs = 2;
     q.sqrt_mask = 1u;
     q.jobs = reinterpret_cast<const vb::PreintJob*>(d + o_jobs);
@@ -1832,39 +1791,34 @@ int ve_debug_imu_factor(const double* noise4, double g_norm, const double* ba, c
     q.p.preint = reinterpret_cast<vb::PreInt*>(d + o_pre);
     vb::BaDims dm{};
     dm.G[2] = g_norm;
-    int rc = VE_OK;
-    bool ok = cudaMemcpy(d + o_seq, &q, sizeof(q), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d + o_jobs, jobs, sizeof(jobs), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d + o_rec, rec.data(), rec.size() * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
-    if (ok && params32) ok = cudaMemcpy(d + o_prm, params32, 32 * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
-    if (ok) {
-        vb::BatchShape sh{};
-        sh.S = 1;
-        sh.W = 0;
-        sh.any_jobs = 1;
-        vb::launch_preint_jobs(reinterpret_cast<vb::BaSeq*>(d + o_seq), sh, nullptr, nullptr, nullptr);
-        if (params32 && out_factor) {
-            vb::launch_debug_imu(dm, reinterpret_cast<const vb::PreInt*>(d + o_pre), reinterpret_cast<const double*>(d + o_prm),
-                                 reinterpret_cast<double*>(d + o_out), nullptr);
-            ok = cudaMemcpy(out_factor, d + o_out, 465 * sizeof(double), cudaMemcpyDeviceToHost) == cudaSuccess;
-        }
-        if (ok && out_preint) {
-            vb::PreInt pre;
-            ok = cudaMemcpy(&pre, d + o_pre, sizeof(pre), cudaMemcpyDeviceToHost) == cudaSuccess;
-            if (ok) {  // sum_dt | dp 3 | dq 4 (wxyz) | dv 3 | jac 225 | cov 225 | sqrt_info 225
-                out_preint[0] = pre.sum_dt;
-                std::memcpy(out_preint + 1, pre.dp, 3 * sizeof(double));
-                std::memcpy(out_preint + 4, pre.dq, 4 * sizeof(double));
-                std::memcpy(out_preint + 8, pre.dv, 3 * sizeof(double));
-                std::memcpy(out_preint + 11, pre.jac, 225 * sizeof(double));
-                std::memcpy(out_preint + 236, pre.cov, 225 * sizeof(double));
-                std::memcpy(out_preint + 461, pre.sqrt_info, 225 * sizeof(double));
-            }
-        }
+    if (cudaMemcpy(d + o_seq, &q, sizeof(q), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(d + o_jobs, jobs, sizeof(jobs), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(d + o_rec, rec.data(), rec.size() * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
+        (params32 && cudaMemcpy(d + o_prm, params32, 32 * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess))
+        return VE_ERR_CUDA;
+    vb::BatchShape sh{};
+    sh.S = 1;
+    sh.W = 0;
+    sh.any_jobs = 1;
+    vb::launch_preint_jobs(reinterpret_cast<vb::BaSeq*>(d + o_seq), sh, nullptr, nullptr, nullptr);
+    if (params32 && out_factor) {
+        vb::launch_debug_imu(dm, reinterpret_cast<const vb::PreInt*>(d + o_pre), reinterpret_cast<const double*>(d + o_prm),
+                             reinterpret_cast<double*>(d + o_out), nullptr);
+        if (cudaMemcpy(out_factor, d + o_out, 465 * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) return VE_ERR_CUDA;
     }
-    if (!ok || cudaGetLastError() != cudaSuccess) rc = VE_ERR_CUDA;
-    cudaFree(d);
-    return rc;
+    if (out_preint) {
+        vb::PreInt pre;
+        if (cudaMemcpy(&pre, d + o_pre, sizeof(pre), cudaMemcpyDeviceToHost) != cudaSuccess) return VE_ERR_CUDA;
+        // sum_dt | dp 3 | dq 4 (wxyz) | dv 3 | jac 225 | cov 225 | sqrt_info 225
+        out_preint[0] = pre.sum_dt;
+        std::memcpy(out_preint + 1, pre.dp, 3 * sizeof(double));
+        std::memcpy(out_preint + 4, pre.dq, 4 * sizeof(double));
+        std::memcpy(out_preint + 8, pre.dv, 3 * sizeof(double));
+        std::memcpy(out_preint + 11, pre.jac, 225 * sizeof(double));
+        std::memcpy(out_preint + 236, pre.cov, 225 * sizeof(double));
+        std::memcpy(out_preint + 461, pre.sqrt_info, 225 * sizeof(double));
+    }
+    return cudaGetLastError() == cudaSuccess ? VE_OK : VE_ERR_CUDA;
 }
 
 }  // extern "C"

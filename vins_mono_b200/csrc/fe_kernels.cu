@@ -6,9 +6,8 @@
 // no FMA contraction where OpenCV's baseline build has none (explicit __fmul_rn/__fadd_rn), integer
 // window sums accumulated exactly.  All of this is HBM/L2-bound byte and integer work; nothing here is
 // GEMM shaped, so no tensor cores.
+#include "cuda_check.h"
 #include "fe_kernels.h"
-
-#include <mutex>
 
 #include <cfloat>
 #include <cstdint>
@@ -727,11 +726,6 @@ __global__ void __launch_bounds__(32) gftt_select_kernel(const FeSeq* __restrict
 
 // ---------------------------------------------------------------------------------------------
 // launch wrappers: one launch per stage for the whole batch (member = last grid dimension)
-namespace {
-std::mutex g_sort_mutex;
-bool g_sort_configured[64] = {};
-}  // namespace
-
 void launch_track(const FeSeq* seqs, const FeShape& sh, cudaStream_t s, int* launches, KernelProfile* prof) {
     KernelProfile none;
     if (!prof) prof = &none;
@@ -814,16 +808,7 @@ void launch_detect(const FeSeq* seqs, const FeShape& sh, const int* halfw, cudaS
     prof->end(4, s);
     prof->begin(s);
     gftt_candidates_kernel<<<dim3((cols + 31) / 32, (rows + 7) / 8, sh.S), dim3(32, 8), 0, s>>>(seqs, rows, cols, 0.01, sh.key_capacity);
-    {
-        std::lock_guard<std::mutex> lock(g_sort_mutex);  // the attribute belongs to the current device
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (!g_sort_configured[dev & 63]) {
-            cudaFuncSetAttribute(sort_keys_desc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 SORT_SMEM_KEYS * (int)sizeof(unsigned long long));
-            g_sort_configured[dev & 63] = true;
-        }
-    }
+    raise_dynamic_smem((const void*)sort_keys_desc_kernel, SORT_SMEM_KEYS * (int)sizeof(unsigned long long));
     sort_keys_desc_kernel<<<sh.S, 1024, SORT_SMEM_KEYS * sizeof(unsigned long long), s>>>(seqs, sh.key_capacity);
     const int cell = (int)lrint((double)sh.min_dist);
     const int gw = (cols + cell - 1) / cell, gh = (rows + cell - 1) / cell;

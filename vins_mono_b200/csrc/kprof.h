@@ -1,22 +1,24 @@
 // Per-kernel device timing for bench.py's roofline object: when enabled, every launch group is bracketed by CUDA
 // events on the launching stream and waited for (so it serialises the pipeline: profile passes are separate from
-// timed passes).
+// timed passes).  The events are created on the device current at enable(): the owning handle's.
 #pragma once
 #include <cuda_runtime.h>
+
+#include "cuda_check.h"
 
 namespace vb {
 
 struct KernelProfile {
     static constexpr int MAX_K = 16;
     bool on = false;
-    cudaEvent_t a = nullptr, b = nullptr;
+    Event a, b;
     double ms[MAX_K] = {};
     int count[MAX_K] = {};
     void enable(bool v) {
         on = v;
         if (v && !a) {
-            cudaEventCreate(&a);
-            cudaEventCreate(&b);
+            a.create();
+            b.create();
         }
         for (int i = 0; i < MAX_K; i++) ms[i] = 0, count[i] = 0;
     }
@@ -31,10 +33,6 @@ struct KernelProfile {
         cudaEventElapsedTime(&t, a, b);
         ms[k] += t;
         count[k] += launches;
-    }
-    ~KernelProfile() {
-        if (a) cudaEventDestroy(a);
-        if (b) cudaEventDestroy(b);
     }
 };
 

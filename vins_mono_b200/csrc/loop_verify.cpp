@@ -6,9 +6,11 @@
 
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
+#include "cuda_check.h"
 #include "host_math.h"
 #include "lv_kernels.h"
 #include "lv_layout.h"
@@ -21,36 +23,25 @@ struct LvState {
     int pattern[4 * LV_BITS] = {};
     int S = 0, cap_kf = 0, device = 0;
     size_t slot_bytes = 0, stage_bytes = 0, conn_bytes = 0, res_doubles = 0;
-    char *d_arena = nullptr, *d_stage = nullptr, *h_stage = nullptr, *d_ascratch = nullptr, *d_cscratch = nullptr;
-    int* d_pattern = nullptr;
-    int* h_status = nullptr;
-    long long *h_jobs = nullptr, *d_jobs = nullptr;
-    double *h_res = nullptr, *d_res = nullptr;
+    DeviceArray<char> d_arena, d_stage, d_ascratch, d_cscratch;
+    PinnedArray<char> h_stage;
+    DeviceArray<int> d_pattern;
+    PinnedArray<int> h_status;
+    PinnedArray<long long> h_jobs;
+    DeviceArray<long long> d_jobs;
+    PinnedArray<double> h_res;
+    DeviceArray<double> d_res;
     std::vector<char> attached;  // per slot, host copy of the slot header's flag
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev[8] = {};
+    Stream stream;
+    Event ev[8];  // 0-3 around the attach stages, 4-7 around the verification stages
     float ms[6] = {0, 0, 0, 0, 0, 0};
+    ~LvState() {  // the buffers go once the stream has drained
+        cudaSetDevice(device);
+        if (stream) cudaStreamSynchronize(stream);
+    }
 };
 
-void lv_release(LvState* s) {
-    if (!s) return;
-    if (s->stream) cudaStreamSynchronize(s->stream);
-    cudaFree(s->d_arena);
-    cudaFree(s->d_stage);
-    cudaFree(s->d_ascratch);
-    cudaFree(s->d_cscratch);
-    cudaFree(s->d_pattern);
-    cudaFree(s->d_jobs);
-    cudaFree(s->d_res);
-    cudaFreeHost(s->h_stage);
-    cudaFreeHost(s->h_status);
-    cudaFreeHost(s->h_jobs);
-    cudaFreeHost(s->h_res);
-    for (cudaEvent_t e : s->ev)
-        if (e) cudaEventDestroy(e);
-    if (s->stream) cudaStreamDestroy(s->stream);
-    delete s;
-}
+void lv_release(LvState* s) { delete s; }
 
 }  // namespace vb
 
@@ -65,6 +56,31 @@ bool config_ok(const vp_loop_config* c) {
     return true;
 }
 
+// The stream, events and buffers of a state whose sizes are set, on its device.
+int create_resources(LvState* s, std::string* err) {
+    const vp_loop_config* c = &s->cfg;
+    const size_t S = (size_t)s->S;
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->stream.create());
+    for (vb::Event& ev : s->ev) VB_CUDA_CHECK(err, VP_ERR_CUDA, ev.create());
+    const size_t arena = vb::lv_arena_bytes(s->S, s->cap_kf, c->max_window, c->max_corners);
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_arena.alloc(arena));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemset(s->d_arena, 0, arena));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_stage.alloc(s->stage_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_stage.alloc(s->stage_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_ascratch.alloc(vb::lv_attach_layout(c->rows, c->cols).total));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_status.alloc(4));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_cscratch.alloc(S * s->conn_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemset(s->d_cscratch, 0, S * s->conn_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_pattern.alloc(4 * vb::LV_BITS));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy(s->d_pattern, s->pattern, sizeof(s->pattern), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_jobs.alloc(S * 2));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_jobs.alloc(S * 2));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_res.alloc(S * s->res_doubles));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_res.alloc(S * s->res_doubles));
+    return 0;
+}
+
 int enable(LvState** slot, const vp_loop_config* c, int S, int cap_kf, int device, std::string* err) {
     if (!config_ok(c)) {
         *err = "vp_loop_enable: invalid configuration";
@@ -74,7 +90,7 @@ int enable(LvState** slot, const vp_loop_config* c, int S, int cap_kf, int devic
         *err = "vp_loop_enable: loop verification is already enabled";
         return VP_ERR_INVALID;
     }
-    LvState* s = new LvState;
+    std::unique_ptr<LvState> s(new LvState);
     s->cfg = *c;
     s->cfg.brief_pattern = nullptr;
     std::memcpy(s->pattern, c->brief_pattern, sizeof(s->pattern));
@@ -86,42 +102,38 @@ int enable(LvState** slot, const vp_loop_config* c, int S, int cap_kf, int devic
     s->conn_bytes = vb::lv_conn_layout(c->max_window).total;
     s->res_doubles = vb::lv_result_doubles(c->max_window);
     s->attached.assign((size_t)S * cap_kf, 0);
-    auto fail = [&](cudaError_t e) {
-        *err = std::string("vp_loop_enable: ") + cudaGetErrorString(e);
-        cudaGetLastError();
-        vb::lv_release(s);
-        return e == cudaErrorMemoryAllocation ? VP_ERR_CAPACITY : VP_ERR_CUDA;
-    };
-    cudaError_t e;
-    if ((e = cudaSetDevice(device)) != cudaSuccess) return fail(e);
-    if ((e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
-    for (cudaEvent_t& ev : s->ev)
-        if ((e = cudaEventCreate(&ev)) != cudaSuccess) return fail(e);
-    const size_t arena = vb::lv_arena_bytes(S, cap_kf, c->max_window, c->max_corners);
-    if ((e = cudaMalloc((void**)&s->d_arena, arena)) != cudaSuccess) return fail(e);
-    if ((e = cudaMemset(s->d_arena, 0, arena)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_stage, s->stage_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&s->h_stage, s->stage_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_ascratch, vb::lv_attach_layout(c->rows, c->cols).total)) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&s->h_status, 16)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_cscratch, (size_t)S * s->conn_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMemset(s->d_cscratch, 0, (size_t)S * s->conn_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_pattern, sizeof(s->pattern))) != cudaSuccess) return fail(e);
-    if ((e = cudaMemcpy(s->d_pattern, s->pattern, sizeof(s->pattern), cudaMemcpyHostToDevice)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_jobs, (size_t)S * 2 * sizeof(long long))) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&s->h_jobs, (size_t)S * 2 * sizeof(long long))) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&s->d_res, (size_t)S * s->res_doubles * sizeof(double))) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&s->h_res, (size_t)S * s->res_doubles * sizeof(double))) != cudaSuccess) return fail(e);
-    *slot = s;
+    const int rc = create_resources(s.get(), err);
+    // the failure is also the thread's last CUDA error: cleared here; an allocation that does not fit is a capacity error
+    if (rc) return cudaGetLastError() == cudaErrorMemoryAllocation ? VP_ERR_CAPACITY : rc;
+    *slot = s.release();
     return 0;
 }
 
-// Drains the stream after a failed call so that the next call starts clean.
-int cuda_fail(LvState* s, std::string* err, const char* what, cudaError_t e) {
-    *err = std::string(what) + ": " + cudaGetErrorString(e);
-    cudaStreamSynchronize(s->stream);
-    cudaGetLastError();
-    return VP_ERR_CUDA;
+// After a failed call the stream may hold part of a launch chain: it is drained so that the next call starts clean.
+int drain_on_error(LvState* s, int rc) {
+    if (rc) {
+        cudaStreamSynchronize(s->stream);
+        cudaGetLastError();
+    }
+    return rc;
+}
+
+// One staged key frame into arena slot `slot`: the input copy, the attach chain, the status copy, then a wait.
+int attach_chain(LvState* s, size_t slot, std::string* err) {
+    const vp_loop_config& c = s->cfg;
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_stage, s->h_stage, s->stage_bytes, cudaMemcpyHostToDevice, s->stream));
+    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, s->d_arena + slot * s->slot_bytes, s->d_pattern,
+                         c.rows, c.cols, c.max_window, c.max_corners, {}};
+    std::memcpy(L.intrinsics, c.intrinsics, sizeof(L.intrinsics));
+    cudaEvent_t ev[4] = {s->ev[0], s->ev[1], s->ev[2], s->ev[3]};
+    vb::launch_lv_attach(L, s->stream, ev);
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaGetLastError());
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->h_status, s->d_ascratch + vb::lv_attach_layout(c.rows, c.cols).status, 8,
+                                                    cudaMemcpyDeviceToHost, s->stream));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaStreamSynchronize(s->stream));
+    for (int k = 0; k < 3; k++) cudaEventElapsedTime(&s->ms[k], s->ev[k], s->ev[k + 1]);
+    return 0;
 }
 
 int attach(LvState* s, int member, int index, const double* P3, const double* Q4, const uint8_t* img, size_t stride, int n,
@@ -149,26 +161,32 @@ int attach(LvState* s, int member, int index, const double* P3, const double* Q4
         std::memcpy(s->h_stage + st.norm, norm, 8 * (size_t)n);
         std::memcpy(s->h_stage + st.id, ids, 8 * (size_t)n);
     }
-    cudaError_t e;
-    if ((e = cudaSetDevice(s->device)) != cudaSuccess) return cuda_fail(s, err, "cudaSetDevice", e);
-    if ((e = cudaMemcpyAsync(s->d_stage, s->h_stage, s->stage_bytes, cudaMemcpyHostToDevice, s->stream)) != cudaSuccess)
-        return cuda_fail(s, err, "attach input copy", e);
-    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, s->d_arena + ((size_t)member * s->cap_kf + index) * s->slot_bytes, s->d_pattern,
-                         c.rows, c.cols, c.max_window, c.max_corners, {}};
-    std::memcpy(L.intrinsics, c.intrinsics, sizeof(L.intrinsics));
-    vb::launch_lv_attach(L, s->stream, s->ev);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(s, err, "attach launch chain", e);
-    if ((e = cudaMemcpyAsync(s->h_status, s->d_ascratch + vb::lv_attach_layout(c.rows, c.cols).status, 8, cudaMemcpyDeviceToHost,
-                             s->stream)) != cudaSuccess)
-        return cuda_fail(s, err, "attach status copy", e);
-    if ((e = cudaStreamSynchronize(s->stream)) != cudaSuccess) return cuda_fail(s, err, "attach", e);
-    for (int k = 0; k < 3; k++) cudaEventElapsedTime(&s->ms[k], s->ev[k], s->ev[k + 1]);
+    const int rc = drain_on_error(s, attach_chain(s, (size_t)member * s->cap_kf + index, err));
+    if (rc) return rc;
     if (n_corners) *n_corners = s->h_status[0];
     if (s->h_status[1]) {
         *err = "vp_attach_keyframe: " + std::to_string(s->h_status[0]) + " FAST corners, at most max_corners = " + std::to_string(c.max_corners);
         return VP_ERR_CAPACITY;
     }
     s->attached[(size_t)member * s->cap_kf + index] = 1;
+    return 0;
+}
+
+// The job copy, the verification chain of `jobs` pairs, the result copy, then a wait.
+int connect_chain(LvState* s, int jobs, int match, std::string* err) {
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_jobs, s->h_jobs, (size_t)jobs * 2 * sizeof(long long), cudaMemcpyHostToDevice, s->stream));
+    vb::LvConnLaunch L{s->d_arena, s->d_jobs, s->d_cscratch, s->conn_bytes, s->d_res, s->res_doubles, jobs, s->cfg.max_window,
+                       s->cfg.max_corners, {}, {}};
+    std::memcpy(L.ric, s->cfg.ric9, sizeof(L.ric));
+    std::memcpy(L.tic, s->cfg.tic3, sizeof(L.tic));
+    cudaEvent_t ev[4] = {s->ev[4], s->ev[5], s->ev[6], s->ev[7]};
+    vb::launch_lv_connect(L, s->stream, ev, match);
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaGetLastError());
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->h_res, s->d_res, (size_t)jobs * s->res_doubles * sizeof(double),
+                                                    cudaMemcpyDeviceToHost, s->stream));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaStreamSynchronize(s->stream));
+    for (int k = 0; k < 3; k++) cudaEventElapsedTime(&s->ms[3 + k], s->ev[4 + k], s->ev[5 + k]);
     return 0;
 }
 
@@ -194,21 +212,8 @@ int connect(LvState* s, const int* cur, const int* old, vp_loop_result* r, int c
         jobs++;
     }
     if (!jobs) return 0;
-    cudaError_t e;
-    if ((e = cudaSetDevice(s->device)) != cudaSuccess) return cuda_fail(s, err, "cudaSetDevice", e);
-    if ((e = cudaMemcpyAsync(s->d_jobs, s->h_jobs, (size_t)jobs * 2 * sizeof(long long), cudaMemcpyHostToDevice, s->stream)) != cudaSuccess)
-        return cuda_fail(s, err, "job copy", e);
-    vb::LvConnLaunch L{s->d_arena, s->d_jobs, s->d_cscratch, s->conn_bytes, s->d_res, s->res_doubles, jobs, s->cfg.max_window,
-                       s->cfg.max_corners, {}, {}};
-    std::memcpy(L.ric, s->cfg.ric9, sizeof(L.ric));
-    std::memcpy(L.tic, s->cfg.tic3, sizeof(L.tic));
-    vb::launch_lv_connect(L, s->stream, s->ev + 4, match);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(s, err, "verification launch chain", e);
-    if ((e = cudaMemcpyAsync(s->h_res, s->d_res, (size_t)jobs * s->res_doubles * sizeof(double), cudaMemcpyDeviceToHost, s->stream)) !=
-        cudaSuccess)
-        return cuda_fail(s, err, "result copy", e);
-    if ((e = cudaStreamSynchronize(s->stream)) != cudaSuccess) return cuda_fail(s, err, "verification", e);
-    for (int k = 0; k < 3; k++) cudaEventElapsedTime(&s->ms[3 + k], s->ev[4 + k], s->ev[5 + k]);
+    const int rc = drain_on_error(s, connect_chain(s, jobs, match, err));
+    if (rc) return rc;
     for (int j = 0; j < jobs; j++) {
         const int k = member[j];
         const double* o = s->h_res + (size_t)j * s->res_doubles;
@@ -241,9 +246,7 @@ struct DebugState {
     std::string err;
     int rc = 0;
     DebugState(int rows, int cols, const int* pattern, int max_window, int max_corners) {
-        int ndev = 0;
-        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-            cudaGetLastError();
+        if (!vb::device_available(0)) {
             rc = VP_ERR_NO_DEVICE;
             return;
         }
@@ -396,11 +399,10 @@ int vp_debug_match(int na, const uint64_t* a, int nb, const uint64_t* b, int* id
     h0.vio_Q[0] = h1.vio_Q[0] = 1;
     h1.n_corners = nb;
     h0.attached = h1.attached = 1;
-    bool ok = cudaMemcpy(d.slot(0), &h0, sizeof(h0), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(1), &h1, sizeof(h1), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(0) + sl.wdesc, a, 32 * (size_t)na, cudaMemcpyHostToDevice) == cudaSuccess &&
-              (!nb || cudaMemcpy(d.slot(1) + sl.kdesc, b, 32 * (size_t)nb, cudaMemcpyHostToDevice) == cudaSuccess);
-    if (!ok) return VP_ERR_CUDA;
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(0), &h0, sizeof(h0), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(1), &h1, sizeof(h1), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(0) + sl.wdesc, a, 32 * (size_t)na, cudaMemcpyHostToDevice));
+    if (nb) VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(1) + sl.kdesc, b, 32 * (size_t)nb, cudaMemcpyHostToDevice));
     d.s->attached[0] = d.s->attached[1] = 1;
     const int cur = 0, old = 1;
     vp_loop_result r{};
@@ -424,15 +426,14 @@ int vp_debug_pnp(int n, const float* point_3d, const float* norm, double* Rt12, 
     std::vector<double> ids(n);
     std::vector<int> iota(n);
     for (int i = 0; i < n; i++) ids[i] = iota[i] = i;
-    bool ok = cudaMemcpy(d.slot(0), &h0, sizeof(h0), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(1), &h1, sizeof(h1), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(0) + sl.p3d, point_3d, 12 * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(0) + sl.id, ids.data(), 8 * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.slot(1) + sl.kpn, norm, 8 * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.s->d_cscratch, &n, sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.s->d_cscratch + cl.win_match, iota.data(), 4 * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(d.s->d_cscratch + cl.midx, iota.data(), 4 * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess;
-    if (!ok) return VP_ERR_CUDA;
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(0), &h0, sizeof(h0), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(1), &h1, sizeof(h1), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(0) + sl.p3d, point_3d, 12 * (size_t)n, cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(0) + sl.id, ids.data(), 8 * (size_t)n, cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.slot(1) + sl.kpn, norm, 8 * (size_t)n, cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.s->d_cscratch, &n, sizeof(int), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.s->d_cscratch + cl.win_match, iota.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpy(d.s->d_cscratch + cl.midx, iota.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
     d.s->attached[0] = d.s->attached[1] = 1;
     const int cur = 0, old = 1;
     vp_loop_result r{};

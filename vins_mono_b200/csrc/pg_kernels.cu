@@ -24,13 +24,13 @@
 //                  tile per CTA on FP64 tensor cores), per panel of 64 columns pg_panel_kernel (diagonal tile and the
 //                  panel's row) and pg_tile_kernel<true> (the trailing update, the same tile product), then
 //                  pg_solve_large_kernel (blocked backward solve and the chain's back-substitution).
+#include "cuda_check.h"
 #include "pg_kernels.h"
 #include "pg_layout.h"
 
 #include <algorithm>
 #include <cfloat>
 #include <climits>
-#include <mutex>
 
 #include "ba_device.cuh"
 #include "chol_packed.cuh"
@@ -892,28 +892,13 @@ __global__ void pg_debug_edge_kernel(const double* prm, const double* meas, int 
 
 }  // namespace
 
-namespace {
-// pg_solve_kernel's dynamic shared memory (the Cholesky panel) is above the 48 KB default together with its static part,
-// and so is pg_panel_kernel's: the opt-in is a per-device function attribute, set once per device.
-std::mutex g_pg_cfg_mutex;
-bool g_pg_configured[64];
-
-cudaError_t configure_device(size_t panel) {
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    std::lock_guard<std::mutex> lock(g_pg_cfg_mutex);
-    if (g_pg_configured[dev & 63]) return cudaSuccess;
-    e = cudaFuncSetAttribute(pg_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)panel);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(pg_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PG_PANEL_SMEM);
-    if (e == cudaSuccess) g_pg_configured[dev & 63] = true;
-    return e;
-}
-}  // namespace
-
 int launch_pg_optimize(const PgLaunch& L, cudaStream_t s) {
+    // pg_solve_kernel's dynamic shared memory (the Cholesky panel) is above the 48 KB default together with its static
+    // part, and so is pg_panel_kernel's
     const size_t panel = sizeof(double) * CHOL_NB * CHOL_PS;
-    if (configure_device(panel) != cudaSuccess) return -1;
+    if (raise_dynamic_smem((const void*)pg_solve_kernel, (int)panel) != cudaSuccess ||
+        raise_dynamic_smem((const void*)pg_panel_kernel, (int)PG_PANEL_SMEM) != cudaSuccess)
+        return -1;
     const int T = (std::min(L.max_D, PG_MAX_D) + 1 + 31) / 32;
     const int Tl = pg_tile_np(L.max_D) / PG_TILE;  // panels of the multi-CTA path, 0 when no member takes it
     const int chain_ctas = (L.max_D + 1 + 383) / 384;

@@ -8,6 +8,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -73,11 +74,13 @@ struct vp_batch {
     int cap_anchors = 0;  // free loop anchors an optimised range may hold (vp_config::max_anchors, 0 = PG_MAX_ANCHORS)
     std::string err;
     std::vector<vp_graph*> members;
-    char *h_in = nullptr, *d_in = nullptr;
-    double *h_out = nullptr, *d_out = nullptr, *d_work = nullptr;
+    vb::PinnedArray<char> h_in;
+    vb::DeviceArray<char> d_in;
+    vb::PinnedArray<double> h_out;
+    vb::DeviceArray<double> d_out, d_work;
     size_t work_stride = 0, in_bytes = 0, out_doubles = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    vb::Stream stream;
+    vb::Event ev0, ev1;
     bool busy = false;
     std::vector<int> slots;            // members of the launch in flight, by slot
     std::vector<long long> slot_out;   // their output offsets (doubles)
@@ -154,59 +157,42 @@ int collect(vp_graph* g) {
 }
 
 void release(vp_batch* b) {
+    cudaSetDevice(b->cfg.device);
     vb::lv_release(b->lv);
     if (b->stream) cudaStreamSynchronize(b->stream);
-    cudaFreeHost(b->h_in);
-    cudaFreeHost(b->h_out);
-    cudaFree(b->d_in);
-    cudaFree(b->d_out);
-    cudaFree(b->d_work);
-    if (b->ev0) cudaEventDestroy(b->ev0);
-    if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->stream) cudaStreamDestroy(b->stream);
     for (vp_graph* g : b->members) delete g;
     delete b;
 }
 
-int batch_create(const vp_config* cfg, int n, vp_batch** out, std::string* err) {
+int batch_create(const vp_config* cfg, int n, vp_batch** out) {
     *out = nullptr;
     if (!cfg || n < 1 || cfg->max_keyframes < 2 || cfg->max_anchors < 0 || cfg->max_anchors > vb::PG_CAP_ANCHORS) return VP_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device < 0 || cfg->device >= ndev) {
-        cudaGetLastError();
-        if (err) *err = "no CUDA device";
-        return VP_ERR_NO_DEVICE;
-    }
-    vp_batch* b = new vp_batch;
+    if (!vb::device_available(cfg->device)) return VP_ERR_NO_DEVICE;
+    std::unique_ptr<vp_batch, void (*)(vp_batch*)> b(new vp_batch, release);
     b->cfg = *cfg;
     b->S = n;
     b->cap_anchors = cfg->max_anchors ? cfg->max_anchors : vb::PG_MAX_ANCHORS;
-    auto fail = [&](cudaError_t e) {
-        if (err) *err = cudaGetErrorString(e);
-        release(b);
-        return VP_ERR_CUDA;
-    };
-    cudaError_t e = cudaSetDevice(cfg->device);
-    if (e != cudaSuccess) return fail(e);
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaSetDevice(cfg->device));
     const int cap = cfg->max_keyframes;
     b->work_stride = (vb::pg_work_layout(cap, b->cap_anchors).total + 1) & ~(size_t)1;
     b->in_bytes = vb::pg_arena_bytes(n, cap, b->cap_anchors);
     b->out_doubles = (size_t)n * vb::pg_out_layout(cap).total;
-    if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
-    if ((e = cudaEventCreate(&b->ev0)) != cudaSuccess || (e = cudaEventCreate(&b->ev1)) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&b->h_in, b->in_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMallocHost((void**)&b->h_out, b->out_doubles * sizeof(double))) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&b->d_in, b->in_bytes)) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&b->d_out, b->out_doubles * sizeof(double))) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc((void**)&b->d_work, (size_t)n * b->work_stride * sizeof(double))) != cudaSuccess) return fail(e);
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->stream.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev0.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev1.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_in.alloc(b->in_bytes));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_out.alloc(b->out_doubles));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_in.alloc(b->in_bytes));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_out.alloc(b->out_doubles));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_work.alloc((size_t)n * b->work_stride));
     for (int k = 0; k < n; k++) {
         vp_graph* g = new vp_graph;
-        g->owner = b;
+        g->owner = b.get();
         g->member = k;
         g->cfg = *cfg;
         b->members.push_back(g);
     }
-    *out = b;
+    *out = b.release();
     return 0;
 }
 
@@ -274,29 +260,19 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, st
     return 0;
 }
 
-// One host-to-device copy of the packed arena, the launch chain, one device-to-host copy of the outputs.  On an error
-// the stream may hold part of the chain; it is drained so that a later launch starts clean.
+// One host-to-device copy of the packed arena, the launch chain, one device-to-host copy of the outputs.
 int enqueue(vp_batch* b, size_t in_bytes, size_t out_doubles, int count, int max_n, int max_D) {
     b->t0 = std::chrono::steady_clock::now();
-    auto fail = [&](const char* what, cudaError_t e) {
-        b->err = std::string(what) + ": " + cudaGetErrorString(e);
-        cudaStreamSynchronize(b->stream);
-        cudaGetLastError();
-        return VP_ERR_CUDA;
-    };
-    cudaError_t e;
-    if ((e = cudaSetDevice(b->cfg.device)) != cudaSuccess) return fail("cudaSetDevice", e);
-    if ((e = cudaMemcpyAsync(b->d_in, b->h_in, in_bytes, cudaMemcpyHostToDevice, b->stream)) != cudaSuccess) return fail("input copy", e);
-    if ((e = cudaEventRecord(b->ev0, b->stream)) != cudaSuccess) return fail("cudaEventRecord", e);
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaSetDevice(b->cfg.device));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaMemcpyAsync(b->d_in, b->h_in, in_bytes, cudaMemcpyHostToDevice, b->stream));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaEventRecord(b->ev0, b->stream));
     vb::PgLaunch L{b->d_in,           b->d_work, b->work_stride, b->d_out, b->S, b->cfg.max_keyframes,
                    b->cap_anchors, count,     max_n,          max_D,    PG_MAX_ITERATIONS};
     const int launches = vb::launch_pg_optimize(L, b->stream);
-    e = cudaGetLastError();
-    if (launches < 0 && e == cudaSuccess) e = cudaErrorInvalidConfiguration;
-    if (e != cudaSuccess) return fail("pose-graph launch chain", e);
-    if ((e = cudaEventRecord(b->ev1, b->stream)) != cudaSuccess) return fail("cudaEventRecord", e);
-    if ((e = cudaMemcpyAsync(b->h_out, b->d_out, out_doubles * sizeof(double), cudaMemcpyDeviceToHost, b->stream)) != cudaSuccess)
-        return fail("output copy", e);
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaGetLastError());  // incl. the failed opt-in of a chain that was not launched
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, launches < 0 ? cudaErrorInvalidConfiguration : cudaSuccess);
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaEventRecord(b->ev1, b->stream));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaMemcpyAsync(b->h_out, b->d_out, out_doubles * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
     b->launches = launches;
     return 0;
 }
@@ -345,9 +321,12 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
         count++;
     }
     if (!count) return first_err;
-    reinterpret_cast<int*>(b->h_in)[0] = count;
+    reinterpret_cast<int*>(b->h_in.get())[0] = count;
     const int rc = enqueue(b, off, out_off, count, max_n, max_D);
     if (rc) {  // nothing was committed: every member keeps its pending optimisation
+        // the stream may hold part of the chain: it is drained so that a later launch starts clean
+        cudaStreamSynchronize(b->stream);
+        cudaGetLastError();
         for (const Slot& sl : slots) {
             if (status) status[sl.k] = rc;
             b->members[sl.k]->err = b->err;
@@ -403,7 +382,7 @@ extern "C" {
 int vp_create(const vp_config* cfg, vp_graph** out) {
     if (!out) return VP_ERR_INVALID;
     vp_batch* b = nullptr;
-    const int rc = batch_create(cfg, 1, &b, nullptr);
+    const int rc = batch_create(cfg, 1, &b);
     if (rc) return rc;
     b->members[0]->standalone = true;
     *out = b->members[0];
@@ -597,7 +576,7 @@ int vp_last_timing(vp_graph* g, float* ms, int* launches) {
 
 int vp_batch_create(const vp_config* cfg, int n, vp_batch** out) {
     if (!out) return VP_ERR_INVALID;
-    return batch_create(cfg, n, out, nullptr);
+    return batch_create(cfg, n, out);
 }
 void vp_batch_destroy(vp_batch* b) {
     if (b) release(b);
@@ -624,19 +603,13 @@ int vp_batch_last_timing(vp_batch* b, float* ms2, int* launches) {
 
 int vp_debug_four_dof_error(const double* params8, const double* meas6, int weighted, int robust, double* out37) {
     if (!params8 || !meas6 || !out37) return VP_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        return VP_ERR_NO_DEVICE;
-    }
-    double* d = nullptr;
-    if (cudaMalloc((void**)&d, sizeof(double) * (8 + 6 + 37)) != cudaSuccess) return VP_ERR_CUDA;
+    if (!vb::device_available(0)) return VP_ERR_NO_DEVICE;
+    vb::DeviceArray<double> d;
+    if (d.alloc(8 + 6 + 37) != cudaSuccess) return VP_ERR_CUDA;
     cudaMemcpy(d, params8, sizeof(double) * 8, cudaMemcpyHostToDevice);
     cudaMemcpy(d + 8, meas6, sizeof(double) * 6, cudaMemcpyHostToDevice);
     vb::launch_pg_debug_edge(d, d + 8, weighted, robust, d + 14, nullptr);
-    const cudaError_t e = cudaMemcpy(out37, d + 14, sizeof(double) * 37, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    return e == cudaSuccess ? 0 : VP_ERR_CUDA;
+    return cudaMemcpy(out37, d + 14, sizeof(double) * 37, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : VP_ERR_CUDA;
 }
 
 }  // extern "C"

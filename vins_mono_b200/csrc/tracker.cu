@@ -22,6 +22,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -41,7 +42,7 @@ struct Pt {
 };
 
 struct DevicePyramid {
-    uint8_t* base = nullptr;
+    vb::DeviceArray<uint8_t> base;
     vb::PyramidView view{};
 };
 
@@ -96,17 +97,17 @@ struct vt_tracker {
     vt_batch* batch = nullptr;
     int member = 0;
     // device memory of this member
-    uint8_t* d_lut = nullptr;
+    vb::DeviceArray<uint8_t> d_lut;
     DevicePyramid pyr[2];
     int cur = 0;  // pyr[cur] = cur_img pyramid, pyr[cur^1] = forw_img pyramid
-    uint8_t* d_mask = nullptr;
-    uint8_t* d_fisheye = nullptr;
-    uint8_t* owned_fisheye_mask = nullptr;  // host copy read by setMask
-    float* d_eig = nullptr;
-    unsigned long long* d_keys = nullptr;
+    vb::DeviceArray<uint8_t> d_mask;
+    vb::DeviceArray<uint8_t> d_fisheye;
+    std::vector<uint8_t> owned_fisheye_mask;  // host copy read by setMask
+    vb::DeviceArray<float> d_eig;
+    vb::DeviceArray<unsigned long long> d_keys;
     int key_capacity = 0;
-    int* d_cell_cnt = nullptr;
-    short2* d_cell_pts = nullptr;
+    vb::DeviceArray<int> d_cell_cnt;
+    vb::DeviceArray<short2> d_cell_pts;
     // this member's slots in the batch arenas
     uint8_t* d_raw = nullptr;  // frame slot (host-image path)
     uint8_t* h_img = nullptr;
@@ -138,21 +139,21 @@ struct vt_batch {
     bool standalone = false;
     std::vector<vt_tracker*> members;
     std::string err;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    vb::FeSeq* h_seq = nullptr;
-    vb::FeSeq* d_seq = nullptr;
+    vb::Stream stream;
+    vb::Event ev0, ev1;
+    vb::PinnedArray<vb::FeSeq> h_seq;
+    vb::DeviceArray<vb::FeSeq> d_seq;
     int raw_pitch = 0, capacity = 0, nlev = 0;
-    uint8_t* d_raw = nullptr;   // S x rows x raw_pitch
-    uint8_t* h_img = nullptr;   // pinned S x rows x cols
+    vb::DeviceArray<uint8_t> d_raw;   // S x rows x raw_pitch
+    vb::PinnedArray<uint8_t> h_img;   // S x rows x cols
     ArenaLayout ar{};
-    uint8_t* h_up = nullptr;    // pinned up arena
-    uint8_t* d_up = nullptr;
-    uint8_t* h_dn = nullptr;    // pinned down arena
-    uint8_t* d_dn = nullptr;
-    int* d_halfw = nullptr;
+    vb::PinnedArray<uint8_t> h_up;    // up arena
+    vb::DeviceArray<uint8_t> d_up;
+    vb::PinnedArray<uint8_t> h_dn;    // down arena
+    vb::DeviceArray<uint8_t> d_dn;
+    vb::DeviceArray<int> d_halfw;
     vb::KernelProfile prof;  // 0 clahe_lut+apply, 1 pyrdown x3, 2 lk, 3 mask, 4 min_eig, 5 candidates+sort+select
-    vb::HostPool* pool = nullptr;
+    std::unique_ptr<vb::HostPool> pool;
     float last_ms = 0;
     int last_launches = 0;
 };
@@ -173,7 +174,7 @@ int lk_levels(int rows, int cols, int win, int max_level) {
     return lv;
 }
 
-int alloc_pyramid(vt_tracker* t, DevicePyramid& p) {
+cudaError_t alloc_pyramid(const vt_tracker* t, DevicePyramid& p) {
     const int nlev = lk_levels(t->cfg.rows, t->cfg.cols, 21, 3);
     size_t total = 0, offs[vb::MAX_PYR_LEVELS];
     int r = t->cfg.rows, c = t->cfg.cols;
@@ -187,10 +188,10 @@ int alloc_pyramid(vt_tracker* t, DevicePyramid& p) {
         c = (c + 1) / 2;
     }
     p.view.nlev = nlev;
-    VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMalloc(&p.base, total));
+    const cudaError_t e = p.base.alloc(total);
     for (int l = 0; l <= nlev; l++) p.view.img[l] = p.base + offs[l];
     for (int l = nlev + 1; l < vb::MAX_PYR_LEVELS; l++) p.view.img[l] = nullptr;
-    return VT_OK;
+    return e;
 }
 
 // Half widths of cv::circle(..., FILLED) per row offset (midpoint algorithm of OpenCV's Circle()).
@@ -484,7 +485,7 @@ void step_after_track(vt_tracker* t) {
     q.det_pitch = q.forw.pitch[0];
     q.n_centres = kept;
     q.mask = t->d_mask;
-    q.mask_init = t->cfg.fisheye ? t->d_fisheye : nullptr;
+    q.mask_init = t->cfg.fisheye ? t->d_fisheye.get() : nullptr;
     q.centres = t->d.centres;
     q.eig = t->d_eig;
     q.keys = t->d_keys;
@@ -660,23 +661,9 @@ int node_after(vt_tracker* t, bool pub) {
     return 1;
 }
 
-void destroy_member(vt_tracker* t) {
-    if (!t) return;
-    cudaFree(t->d_lut);
-    cudaFree(t->pyr[0].base);
-    cudaFree(t->pyr[1].base);
-    cudaFree(t->d_mask);
-    cudaFree(t->d_fisheye);
-    cudaFree(t->d_eig);
-    cudaFree(t->d_keys);
-    cudaFree(t->d_cell_cnt);
-    cudaFree(t->d_cell_pts);
-    delete[] t->owned_fisheye_mask;
-    delete t;
-}
-
-vt_tracker* create_member(vt_batch* b, int k) {
-    vt_tracker* t = new vt_tracker();
+// Creates member k and appends it to the batch.
+int create_member(vt_batch* b, int k) {
+    std::unique_ptr<vt_tracker> t(new vt_tracker());
     t->cfg = b->cfg;
     t->cfg.fisheye_mask = nullptr;
     t->batch = b;
@@ -686,32 +673,33 @@ vt_tracker* create_member(vt_batch* b, int k) {
     const size_t npx = (size_t)rows * cols;
     t->capacity = b->capacity;
     if (cfg->fisheye) {  // own a copy first: setMask reads it on the host
-        t->owned_fisheye_mask = new uint8_t[npx];
-        std::memcpy(t->owned_fisheye_mask, cfg->fisheye_mask, npx);
-        t->cfg.fisheye_mask = t->owned_fisheye_mask;
+        t->owned_fisheye_mask.assign(cfg->fisheye_mask, cfg->fisheye_mask + npx);
+        t->cfg.fisheye_mask = t->owned_fisheye_mask.data();
     }
-    bool ok = cudaMalloc(&t->d_lut, 64 * 256) == cudaSuccess;
-    ok = ok && alloc_pyramid(t, t->pyr[0]) == VT_OK && alloc_pyramid(t, t->pyr[1]) == VT_OK;
-    ok = ok && cudaMalloc(&t->d_mask, npx) == cudaSuccess && cudaMalloc(&t->d_eig, npx * sizeof(float)) == cudaSuccess;
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_lut.alloc(64 * 256));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, alloc_pyramid(t.get(), t->pyr[0]));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, alloc_pyramid(t.get(), t->pyr[1]));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_mask.alloc(npx));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_eig.alloc(npx));
     t->key_capacity = 1;
     while ((size_t)t->key_capacity < npx / 8) t->key_capacity <<= 1;  // local maxima of a 3x3 NMS: < npx/4 in practice
-    ok = ok && cudaMalloc(&t->d_keys, (size_t)t->key_capacity * sizeof(unsigned long long)) == cudaSuccess;
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_keys.alloc((size_t)t->key_capacity));
     const int cell = cfg->min_dist, gw = (cols + cell - 1) / cell, gh = (rows + cell - 1) / cell;
-    ok = ok && cudaMalloc(&t->d_cell_cnt, (size_t)gw * gh * sizeof(int)) == cudaSuccess &&
-         cudaMalloc(&t->d_cell_pts, (size_t)gw * gh * 8 * sizeof(short2)) == cudaSuccess;
-    if (ok && cfg->fisheye)
-        ok = cudaMalloc(&t->d_fisheye, npx) == cudaSuccess &&
-             cudaMemcpy(t->d_fisheye, t->owned_fisheye_mask, npx, cudaMemcpyHostToDevice) == cudaSuccess;
-    if (!ok) {
-        destroy_member(t);
-        return nullptr;
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_cell_cnt.alloc((size_t)gw * gh));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_cell_pts.alloc((size_t)gw * gh * 8));
+    if (cfg->fisheye) {
+        VB_CUDA_CHECK(b, VT_ERR_CUDA, t->d_fisheye.alloc(npx));
+        VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpy(t->d_fisheye, t->owned_fisheye_mask.data(), npx, cudaMemcpyHostToDevice));
     }
     t->halfw = disc_half_widths(cfg->min_dist);
     t->d_raw = b->d_raw + (size_t)k * rows * b->raw_pitch;
     t->h_img = b->h_img + (size_t)k * npx;
     t->h = arena_slots(b->ar, b->h_up, b->h_dn, k);
     t->d = arena_slots(b->ar, b->d_up, b->d_dn, k);
-    return t;
+    t->cfg.freq = b->cfg.freq;
+    t->cfg.focal_length = b->cfg.focal_length;
+    b->members.push_back(t.release());
+    return VT_OK;
 }
 
 }  // namespace
@@ -724,49 +712,40 @@ int vt_batch_create(const vt_config* cfg, int n, vt_batch** out) {
     if (cfg->rows < 32 || cfg->cols < 32 || cfg->max_cnt <= 0 || cfg->min_dist < 1 ||
         cfg->camera_model < VT_CAMERA_PINHOLE || cfg->camera_model > VT_CAMERA_KANNALA_BRANDT || (cfg->fisheye && !cfg->fisheye_mask))
         return VT_ERR_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev)
-        return VT_ERR_NO_DEVICE;
-    vt_batch* b = new vt_batch();
+    if (!vb::device_available(cfg->device)) return VT_ERR_NO_DEVICE;
+    std::unique_ptr<vt_batch, void (*)(vt_batch*)> b(new vt_batch(), vt_batch_destroy);
     b->cfg = *cfg;
     if (b->cfg.freq == 0) b->cfg.freq = 100;
     if (b->cfg.focal_length == 0) b->cfg.focal_length = 460;
     b->S = n;
-    auto fail = [&](int code) {
-        vt_batch_destroy(b);
-        return code;
-    };
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaSetDevice(cfg->device));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaEventCreate(&b->ev0));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaEventCreate(&b->ev1));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaSetDevice(cfg->device));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->stream.create());
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->ev0.create());
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->ev1.create());
     const int rows = cfg->rows, cols = cfg->cols;
     const size_t npx = (size_t)rows * cols, S = (size_t)n;
     b->raw_pitch = align_up(cols, 64);
     b->capacity = std::max(cfg->max_cnt, 16);
     b->nlev = lk_levels(rows, cols, 21, 3);
     b->ar = arena_layout(S, (size_t)b->capacity);
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_raw, S * rows * b->raw_pitch));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_img, S * npx, cudaHostAllocDefault));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_up, b->ar.up_bytes));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_up, b->ar.up_bytes, cudaHostAllocDefault));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_dn, b->ar.dn_bytes));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_dn, b->ar.dn_bytes, cudaHostAllocDefault));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_seq, sizeof(vb::FeSeq) * S));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaHostAlloc(&b->h_seq, sizeof(vb::FeSeq) * S, cudaHostAllocDefault));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->d_raw.alloc(S * rows * b->raw_pitch));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->h_img.alloc(S * npx));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->d_up.alloc(b->ar.up_bytes));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->h_up.alloc(b->ar.up_bytes));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->d_dn.alloc(b->ar.dn_bytes));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->h_dn.alloc(b->ar.dn_bytes));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->d_seq.alloc(S));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->h_seq.alloc(S));
     std::memset(b->h_seq, 0, sizeof(vb::FeSeq) * S);
     const std::vector<int> hw = disc_half_widths(cfg->min_dist);
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMalloc(&b->d_halfw, hw.size() * sizeof(int)));
-    VB_CUDA_CHECK(b, fail(VT_ERR_CUDA), cudaMemcpy(b->d_halfw, hw.data(), hw.size() * sizeof(int), cudaMemcpyHostToDevice));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, b->d_halfw.alloc(hw.size()));
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaMemcpy(b->d_halfw, hw.data(), hw.size() * sizeof(int), cudaMemcpyHostToDevice));
     for (int k = 0; k < n; k++) {
-        vt_tracker* t = create_member(b, k);
-        if (!t) return fail(VT_ERR_CUDA);
-        t->cfg.freq = b->cfg.freq;
-        t->cfg.focal_length = b->cfg.focal_length;
-        b->members.push_back(t);
+        const int rc = create_member(b.get(), k);
+        if (rc) return rc;
     }
-    b->pool = new vb::HostPool(vb::HostPool::default_workers(n));
-    *out = b;
+    b->pool.reset(new vb::HostPool(vb::HostPool::default_workers(n)));
+    *out = b.release();
     return VT_OK;
 }
 
@@ -774,13 +753,8 @@ void vt_batch_destroy(vt_batch* b) {
     if (!b) return;
     cudaSetDevice(b->cfg.device);
     if (b->stream) cudaStreamSynchronize(b->stream);
-    delete b->pool;
-    for (auto* t : b->members) destroy_member(t);
-    cudaFree(b->d_raw); cudaFree(b->d_up); cudaFree(b->d_dn); cudaFree(b->d_seq); cudaFree(b->d_halfw);
-    cudaFreeHost(b->h_img); cudaFreeHost(b->h_up); cudaFreeHost(b->h_dn); cudaFreeHost(b->h_seq);
-    if (b->ev0) cudaEventDestroy(b->ev0);
-    if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->stream) cudaStreamDestroy(b->stream);
+    b->pool.reset();
+    for (auto* t : b->members) delete t;
     delete b;
 }
 
@@ -831,6 +805,7 @@ int vt_batch_last_timing(const vt_batch* b, float* device_ms, int* kernel_launch
 
 int vt_batch_set_profile(vt_batch* b, int on) {
     if (!b) return VT_ERR_INVALID;
+    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaSetDevice(b->cfg.device));
     b->prof.enable(on != 0);
     return VT_OK;
 }
@@ -1002,10 +977,10 @@ int vt_debug_gftt(vt_tracker* t, const uint8_t* img, size_t row_stride, const ui
     vt_batch* b = t->batch;
     VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaSetDevice(t->cfg.device));
     const int rows = t->cfg.rows, cols = t->cfg.cols;
-    uint8_t* d_user_mask = nullptr;
+    vb::DeviceArray<uint8_t> d_user_mask;
     VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpy2DAsync(t->d_raw, b->raw_pitch, img, row_stride, cols, rows, cudaMemcpyHostToDevice, b->stream));
     if (mask) {
-        VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMalloc(&d_user_mask, (size_t)rows * cols));
+        VB_CUDA_CHECK(t, VT_ERR_CUDA, d_user_mask.alloc((size_t)rows * cols));
         VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaMemcpyAsync(d_user_mask, mask, (size_t)rows * cols, cudaMemcpyHostToDevice, b->stream));
     }
     vb::FeSeq& q = b->h_seq[t->member];
@@ -1032,7 +1007,6 @@ int vt_debug_gftt(vt_tracker* t, const uint8_t* img, size_t row_stride, const ui
                             cudaMemcpyDeviceToHost, b->stream));
     VB_CUDA_CHECK(t, VT_ERR_CUDA, cudaStreamSynchronize(b->stream));
     q.detect = 0;
-    if (d_user_mask) cudaFree(d_user_mask);
     if (t->h.counts[vb::FE_COUNT_CANDIDATES] > t->key_capacity) {
         t->err = "Shi-Tomasi candidate buffer overflow";
         return VT_ERR_CAPACITY;
