@@ -1,14 +1,16 @@
 """Loop-verification bench: device time per stage of one key-frame attach (blur, FAST, BRIEF) and of one verification
 launch chain (matching, PnP hypotheses, refit) at S = 1 and S = 64 pairs per chain, from the library's CUDA events, plus a
-per-kernel split from torch.profiler (--profile).  Inputs: rendered revisit pairs of harness/loop_revisit.py.  Prints one
-JSON line per measurement; --out also writes them to a file.
+per-kernel split from torch.profiler (--profile).  Inputs: rendered revisit pairs of harness/loop_revisit.py, seen through
+the EuRoC PINHOLE camera or (--camera) the reference's 3dm MEI or cla KANNALA_BRANDT camera; the FAST time includes the
+corner lift.  Prints one JSON line per measurement; --out also writes them to a file.
 
-    python -m harness.loop_verify_bench --reps 20 [--profile] [--out profiles/loop_verify_h100.jsonl]
+    python -m harness.loop_verify_bench --reps 20 [--camera pinhole|mei|kb] [--profile] [--out profiles/loop_verify_h100.jsonl]
 """
 from __future__ import annotations
 
 import argparse
 import json
+import os
 import subprocess
 
 import numpy as np
@@ -17,23 +19,14 @@ from harness import loop_revisit, synth
 from oracle import loop_verify as olv
 
 INTR = [synth.FX, synth.FY, synth.CX, synth.CY, synth.K1, synth.K2, synth.P1, synth.P2]
-
-
-def _pair(seq, pts, t_old, t_cur):
-    p, R, *_ = seq.pose(t_cur)
-    _, _, vis = loop_revisit.project(seq, t_cur, pts)
-    ids = np.nonzero(vis)[0]
-    ids = ids[np.linspace(0, len(ids) - 1, min(150, len(ids))).astype(int)]
-    p3d, uv, norm, pid = loop_revisit.window_points(seq, t_cur, ids, pts, p, R)
-    p0, R0, *_ = seq.pose(t_old)
-    return (seq.render(t_old), p0, olv.R_to_quat(R0)), (seq.render(t_cur), p, olv.R_to_quat(R), p3d, uv, norm, pid)
+CAMERA_FILES = {"mei": "3dm/3dm_config.yaml", "kb": "cla/cla_config.yaml"}
 
 
 def _attach(g, old, cur):
     img, P, Q = old
     g.attach_keyframe(0, P, Q, img, np.zeros((0, 3)), np.zeros((0, 2)), np.zeros((0, 2)), np.zeros(0))
     img, P, Q, p3d, uv, norm, pid = cur
-    g.attach_keyframe(1, P, Q, img, p3d, uv, norm, pid)
+    return g.attach_keyframe(1, P, Q, img, p3d, uv, norm, pid)  # the corners of the attach loop_timing reports
 
 
 def main():
@@ -41,36 +34,47 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--out", default=None)
+    ap.add_argument("--camera", choices=["pinhole", "mei", "kb"], default=None)  # named cameras also report their corner count
     a = ap.parse_args()
+    from vins_mono_b200 import config
     from vins_mono_b200.pose_graph import PoseGraph, PoseGraphBatch, loop_config
-    seq = synth.Sequence(seed=0, duration=12.0)
+    model, xi, tag = 0, 0.0, dict(camera=a.camera) if a.camera else {}
+    if a.camera in (None, "pinhole"):
+        seq = synth.Sequence(seed=0, duration=12.0)
+        intr = INTR
+    else:
+        root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+        kw = config.loop_kwargs(config.load(os.path.join(root, "tests", "golden", "config", CAMERA_FILES[a.camera])))
+        model, xi, intr = kw["camera_model"], kw["xi"], kw["intrinsics"]
+        seq = loop_revisit.CameraSequence(model, intr, xi, seed=0, duration=12.0, rows=kw["rows"], cols=kw["cols"])
     pts = loop_revisit.corner_landmarks(seq, np.arange(0.2, 12.0, 0.5))
-    old, cur = _pair(seq, pts, 1.4, 8.9)  # a revisit of this sequence (2.3 m apart, accepted)
-    cfg = loop_config(seq.rows, seq.cols, INTR, synth.RIC, synth.TIC, olv.load_pattern(), 256, 16384)
+    old, cur = loop_revisit.revisit_pair(seq, pts, 1.4, 8.9)  # a revisit of this sequence (2.3 m apart, accepted)
+    cfg = loop_config(seq.rows, seq.cols, intr, synth.RIC, synth.TIC, olv.load_pattern(), 256, 16384)
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     lines = []
 
     def emit(d):
+        d.update(tag)
         d["gpu"] = gpu
         print(json.dumps(d), flush=True)
         lines.append(d)
 
     g = PoseGraph(max_keyframes=2)
-    g.enable_loop(cfg)
+    g.enable_loop(cfg, model, xi)
     att, ver = [], []
     for r in range(a.reps + 3):
-        _attach(g, old, cur)
+        n_corners = _attach(g, old, cur)
         att.append(g.loop_timing()[:3].copy())
         res = g.find_connection(1, 0)
         ver.append(g.loop_timing()[3:].copy())
     att, ver = np.array(att[3:]), np.array(ver[3:])
     emit(dict(what="attach", S=1, blur_ms=float(att[:, 0].mean()), fast_ms=float(att[:, 1].mean()), brief_ms=float(att[:, 2].mean()),
-              reps=a.reps, n_window=len(cur[4])))
+              reps=a.reps, n_window=len(cur[4]), **({"n_corners": n_corners} if tag else {})))
     emit(dict(what="verify", S=1, match_ms=float(ver[:, 0].mean()), hyp_ms=float(ver[:, 1].mean()), refit_ms=float(ver[:, 2].mean()),
               reps=a.reps, n_matches=res["n_matches"], n_inliers=res["n_inliers"], accepted=res["accepted"]))
     S = 64
     b = PoseGraphBatch(S, max_keyframes=2)
-    b.enable_loop(cfg)
+    b.enable_loop(cfg, model, xi)
     for k in range(S):
         _attach(b[k], old, cur)
     ver = []

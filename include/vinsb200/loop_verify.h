@@ -7,7 +7,8 @@
  *
  *   vp_loop_enable / vp_batch_loop_enable   allocate the descriptor arena: one slot per key frame index (0 ..
  *                            max_keyframes - 1) of every member, resident in device memory.  The BRIEF pattern (256
- *                            pairs x1 y1 x2 y2, support_files/brief_pattern.yml) is copied at this call.  PINHOLE only.
+ *                            pairs x1 y1 x2 y2, support_files/brief_pattern.yml) is copied at this call.  PINHOLE;
+ *                            vp_loop_enable_camera (loop_camera.h) takes MEI and KANNALA_BRANDT cameras.
  *                            Per slot about 12 + 32 + 28 bytes per window point and 48 bytes per corner.
  *   vp_attach_keyframe       the KeyFrame constructor's computeWindowBRIEFPoint + computeBRIEFPoint (:75-113): the image
  *                            (rows x cols, 8-bit), the key frame's VIO pose as created (origin_vio_T / origin_vio_R) and its
@@ -42,7 +43,7 @@ extern "C" {
 
 typedef struct vp_loop_config {
     int rows, cols;            /* image size (ROW, COL): 8 .. 1024 rows, 8 .. 2048 columns */
-    double intrinsics[8];      /* PINHOLE: fx fy cx cy k1 k2 p1 p2 */
+    double intrinsics[8];      /* PINHOLE: fx fy cx cy k1 k2 p1 p2 (other models: loop_camera.h) */
     double ric9[9];            /* camera-to-body rotation qic, row-major */
     double tic3[3];            /* camera-to-body translation tic */
     const int* brief_pattern;  /* 256 x (x1, y1, x2, y2) */
@@ -67,7 +68,7 @@ int vp_attach_keyframe(vp_graph* g, int index, const double* vio_P3, const doubl
                        int* n_corners);
 int vp_find_connection(vp_graph* g, int cur, int old, vp_loop_result* r, int cap, double* match_xyid);
 int vp_batch_find_connection(vp_batch* b, const int* cur, const int* old, vp_loop_result* r, int cap, double* match_xyid, int* status);
-/* ms6 = blur, FAST, BRIEF (last attach) | matching, hypotheses, refit (last verification) */
+/* ms6 = blur, FAST (with the corner lift), BRIEF (last attach) | matching, hypotheses, refit (last verification) */
 int vp_loop_last_timing(vp_graph* g, float* ms6);
 int vp_batch_loop_last_timing(vp_batch* b, float* ms6);
 

@@ -95,6 +95,23 @@ def estimator_kwargs(cfg: dict, max_features: int = 1000) -> dict:
                 tic=tic, ric=ric)
 
 
+def loop_kwargs(cfg: dict, ric=None, tic=None) -> dict:
+    """What loop verification needs from the file (pose_graph_node.cpp reads the same YAML as the tracker): the image size, the
+    camera model, its intrinsics (in vt_config's order for that model) and xi as tracker_kwargs reads them, and qic / tic as
+    estimator_kwargs normalises them.  ric / tic replace the file's extrinsic, e.g. with the estimator's calibration when
+    estimate_extrinsic = 2.
+
+        kw = loop_kwargs(cfg)
+        g.enable_loop(loop_config(kw["rows"], kw["cols"], kw["intrinsics"], kw["ric"], kw["tic"], pattern), kw["camera_model"], kw["xi"])
+    """
+    trk = tracker_kwargs(dict(cfg, fisheye=0))  # the fisheye mask only concerns the tracker
+    est = estimator_kwargs(cfg)
+    return dict(rows=trk["rows"], cols=trk["cols"], camera_model=trk["camera_model"], xi=trk["xi"],
+                intrinsics=[trk[k] for k in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2")],
+                ric=np.asarray(est["ric"] if ric is None else ric, float).reshape(3, 3),
+                tic=np.asarray(est["tic"] if tic is None else tic, float).reshape(3))
+
+
 def ignored(cfg: dict) -> dict:
     """Keys of the file that have no effect here (reported so that nothing is dropped silently)."""
     return {k: cfg[k] for k in ("max_solver_time", "show_track", "loop_closure", "fast_relocalization", "load_previous_pose_graph",

@@ -2,6 +2,9 @@
 // key-frame attach and the verification of candidate pairs around the device stages of lv_kernels.cu.
 #include "vinsb200/loop_verify.h"
 
+#include "vinsb200/loop_camera.h"
+#include "vinsb200/tracker.h"
+
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -10,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "camera_lift.h"
 #include "cuda_check.h"
 #include "host_math.h"
 #include "lv_kernels.h"
@@ -18,8 +22,16 @@
 
 namespace vb {
 
+static_assert((int)VP_CAMERA_PINHOLE == (int)VT_CAMERA_PINHOLE && (int)VP_CAMERA_MEI == (int)VT_CAMERA_MEI &&
+                  (int)VP_CAMERA_KANNALA_BRANDT == (int)VT_CAMERA_KANNALA_BRANDT,
+              "the loop-verification camera models are the tracker's");
+static_assert(VP_CAMERA_PINHOLE == CAM_PINHOLE && VP_CAMERA_MEI == CAM_MEI && VP_CAMERA_KANNALA_BRANDT == CAM_KANNALA_BRANDT,
+              "camera_lift.h model values");
+
 struct LvState {
     vp_loop_config cfg{};
+    int camera_model = VP_CAMERA_PINHOLE;
+    double xi = 0.0;
     int pattern[4 * LV_BITS] = {};
     int S = 0, cap_kf = 0, device = 0;
     size_t slot_bytes = 0, stage_bytes = 0, conn_bytes = 0, res_doubles = 0;
@@ -48,6 +60,10 @@ void lv_release(LvState* s) { delete s; }
 namespace {
 
 using vb::LvState;
+
+bool camera_ok(int camera_model, double xi) {
+    return camera_model >= VP_CAMERA_PINHOLE && camera_model <= VP_CAMERA_KANNALA_BRANDT && std::isfinite(xi);
+}
 
 bool config_ok(const vp_loop_config* c) {
     if (!c || !c->brief_pattern || c->rows < 8 || c->rows > vb::LV_MAX_ROWS || c->cols < 8 || c->cols > vb::LV_MAX_COLS) return false;
@@ -81,8 +97,8 @@ int create_resources(LvState* s, std::string* err) {
     return 0;
 }
 
-int enable(LvState** slot, const vp_loop_config* c, int S, int cap_kf, int device, std::string* err) {
-    if (!config_ok(c)) {
+int enable(LvState** slot, const vp_loop_config* c, int camera_model, double xi, int S, int cap_kf, int device, std::string* err) {
+    if (!config_ok(c) || !camera_ok(camera_model, xi)) {
         *err = "vp_loop_enable: invalid configuration";
         return VP_ERR_INVALID;
     }
@@ -93,6 +109,8 @@ int enable(LvState** slot, const vp_loop_config* c, int S, int cap_kf, int devic
     std::unique_ptr<LvState> s(new LvState);
     s->cfg = *c;
     s->cfg.brief_pattern = nullptr;
+    s->camera_model = camera_model;
+    s->xi = xi;
     std::memcpy(s->pattern, c->brief_pattern, sizeof(s->pattern));
     s->S = S;
     s->cap_kf = cap_kf;
@@ -124,7 +142,7 @@ int attach_chain(LvState* s, size_t slot, std::string* err) {
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_stage, s->h_stage, s->stage_bytes, cudaMemcpyHostToDevice, s->stream));
     vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, s->d_arena + slot * s->slot_bytes, s->d_pattern,
-                         c.rows, c.cols, c.max_window, c.max_corners, {}};
+                         c.rows, c.cols, c.max_window, c.max_corners, {}, s->camera_model, s->xi};
     std::memcpy(L.intrinsics, c.intrinsics, sizeof(L.intrinsics));
     cudaEvent_t ev[4] = {s->ev[0], s->ev[1], s->ev[2], s->ev[3]};
     vb::launch_lv_attach(L, s->stream, ev);
@@ -259,7 +277,7 @@ struct DebugState {
         c.brief_pattern = pattern ? pattern : zero_pattern;
         c.max_window = max_window;
         c.max_corners = max_corners;
-        rc = enable(&s, &c, 1, 2, 0, &err);
+        rc = enable(&s, &c, VP_CAMERA_PINHOLE, 0.0, 1, 2, 0, &err);
     }
     ~DebugState() { vb::lv_release(s); }
     char* slot(int k) const { return s->d_arena + k * s->slot_bytes; }
@@ -271,7 +289,11 @@ const double kIdentityQ[4] = {1, 0, 0, 0}, kZeroP[3] = {0, 0, 0};
 
 extern "C" {
 
-int vp_loop_enable(vp_graph* g, const vp_loop_config* cfg) {
+int vp_loop_enable(vp_graph* g, const vp_loop_config* cfg) { return vp_loop_enable_camera(g, cfg, VP_CAMERA_PINHOLE, 0.0); }
+
+int vp_batch_loop_enable(vp_batch* b, const vp_loop_config* cfg) { return vp_batch_loop_enable_camera(b, cfg, VP_CAMERA_PINHOLE, 0.0); }
+
+int vp_loop_enable_camera(vp_graph* g, const vp_loop_config* cfg, int camera_model, double xi) {
     if (!g) return VP_ERR_INVALID;
     int member = 0, device = 0;
     bool standalone = false;
@@ -281,14 +303,14 @@ int vp_loop_enable(vp_graph* g, const vp_loop_config* cfg) {
         return VP_ERR_INVALID;
     }
     const int cap = vb::pg_capacity(b, &device);
-    return enable(vb::pg_loop_state(b), cfg, 1, cap, device, vb::pg_error(g));
+    return enable(vb::pg_loop_state(b), cfg, camera_model, xi, 1, cap, device, vb::pg_error(g));
 }
 
-int vp_batch_loop_enable(vp_batch* b, const vp_loop_config* cfg) {
+int vp_batch_loop_enable_camera(vp_batch* b, const vp_loop_config* cfg, int camera_model, double xi) {
     if (!b) return VP_ERR_INVALID;
     int device = 0;
     const int cap = vb::pg_capacity(b, &device);
-    return enable(vb::pg_loop_state(b), cfg, vp_batch_size(b), cap, device, vb::pg_batch_error(b));
+    return enable(vb::pg_loop_state(b), cfg, camera_model, xi, vp_batch_size(b), cap, device, vb::pg_batch_error(b));
 }
 
 int vp_attach_keyframe(vp_graph* g, int index, const double* vio_P3, const double* vio_Qwxyz, const uint8_t* img, size_t row_stride,
@@ -450,6 +472,27 @@ int vp_debug_pnp(int n, const float* point_3d, const float* norm, double* Rt12, 
         std::memset(inlier, 0, n);
         for (int i = 0; i < r.n_points; i++) inlier[(int)list[3 * i + 2]] = 1;
     }
+    return 0;
+}
+
+int vp_debug_lift(int camera_model, const double* intrinsics8, double xi, int n, const float* uv, float* xy) {
+    if (!intrinsics8 || !uv || !xy || n < 1 || n > vb::LV_CAP_CORNERS || !camera_ok(camera_model, xi) || !(intrinsics8[0] != 0.0) ||
+        !(intrinsics8[1] != 0.0))
+        return VP_ERR_INVALID;
+    DebugState d(8, 8, nullptr, 1, n);
+    if (d.rc) return d.rc;
+    LvState* s = d.s;
+    const vb::LvSlotLayout sl = vb::lv_slot_layout(1, n);
+    const int status[2] = {n, 0};
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpyAsync(d.slot(0) + sl.kp, uv, 8 * (size_t)n, cudaMemcpyHostToDevice, s->stream));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_ascratch + vb::lv_attach_layout(8, 8).status, status, sizeof(status),
+                                                      cudaMemcpyHostToDevice, s->stream));
+    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, d.slot(0), s->d_pattern, 8, 8, 1, n, {}, camera_model, xi};
+    std::memcpy(L.intrinsics, intrinsics8, sizeof(L.intrinsics));
+    vb::launch_lv_lift(L, s->stream);
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaGetLastError());
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpyAsync(xy, d.slot(0) + sl.kpn, 8 * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaStreamSynchronize(s->stream));
     return 0;
 }
 

@@ -1,12 +1,14 @@
 // Loop verification on the device (KeyFrame::findConnection and what it needs, pose_graph/src/keyframe.cpp):
 //   attach   GaussianBlur 9x9 sigma 2 (OpenCV's 8-bit fixed-point path), FAST-9 + non-maximum suppression (cv::FAST, 20),
-//            ordered corner compaction with liftProjective (PINHOLE), BRIEF on the window points and on the corners
+//            ordered corner compaction, liftProjective of the corners (PINHOLE, MEI, KANNALA_BRANDT: camera_lift.h), BRIEF on
+//            the window points and on the corners
 //   connect  brute-force Hamming matching (searchByBRIEFDes), PnP-RANSAC in float64 (one warp per hypothesis, 6-point
 //            DLT, consensus count, Gauss-Newton refit on the best consensus set), relative pose and the loop gate.
 // Every stage up to the matches is integer (or float32 where the reference is) and bit-exact; no sum uses atomics.  The
 // member / job index is the last grid dimension of every kernel.
 #include <cstdint>
 
+#include "camera_lift.h"
 #include "lv_kernels.h"
 #include "lv_layout.h"
 
@@ -111,33 +113,15 @@ __global__ void lv_fast_nms_kernel(char* scratch, size_t scratch_stride, int row
     if (threadIdx.x == 0) reinterpret_cast<int*>(sc + al.rowcnt)[y] = count;
 }
 
-__device__ __forceinline__ void lift_pinhole(const double* c, double px, double py, double& X, double& Y) {
-    const double fx = c[0], fy = c[1], cx = c[2], cy = c[3], k1 = c[4], k2 = c[5], p1 = c[6], p2 = c[7];
-    const double mx_d = (1.0 / fx) * px + (-cx / fx), my_d = (1.0 / fy) * py + (-cy / fy);
-    double ux = mx_d, uy = my_d;
-    if (!(k1 == 0.0 && k2 == 0.0 && p1 == 0.0 && p2 == 0.0)) {
-        for (int i = 0; i < 8; ++i) {  // the recursive distortion model of PinholeCamera::liftProjective
-            const double x2 = ux * ux, y2 = uy * uy, xy = ux * uy, rho2 = x2 + y2;
-            const double rad = k1 * rho2 + k2 * rho2 * rho2;
-            const double ddx = ux * rad + 2.0 * p1 * xy + p2 * (rho2 + 2.0 * x2);
-            const double ddy = uy * rad + 2.0 * p2 * xy + p1 * (rho2 + 2.0 * y2);
-            ux = mx_d - ddx;
-            uy = my_d - ddy;
-        }
-    }
-    X = ux;
-    Y = uy;
-}
-
 struct Intr {
     double v[9];
 };
 
-// One CTA per attach: exclusive scan of the row counts, then (when the corners fit) the corners in row-major order with
-// their normalised coordinates, the window arrays and the header into the slot.
-__global__ void __launch_bounds__(1024) lv_fast_compact_kernel(const char* stage, char* scratch, char* slot, size_t stage_stride,
+// One CTA per attach: exclusive scan of the row counts, then (when the corners fit) the corners in row-major order, the
+// window arrays and the header into the slot.
+__global__ void __launch_bounds__(1024, 1) lv_fast_compact_kernel(const char* stage, char* scratch, char* slot, size_t stage_stride,
                                                                size_t scratch_stride, size_t slot_stride, int rows, int cols,
-                                                               int max_window, int max_corners, Intr intr) {
+                                                               int max_window, int max_corners) {
     __shared__ int base[LV_MAX_ROWS];
     const LvAttachLayout al = lv_attach_layout(rows, cols);
     const LvStageLayout st = lv_stage_layout(rows, cols, max_window);
@@ -164,7 +148,6 @@ __global__ void __launch_bounds__(1024) lv_fast_compact_kernel(const char* stage
     if (overflow) return;
     const uint8_t* keep = reinterpret_cast<const uint8_t*>(sc + al.keep);
     float* kp = reinterpret_cast<float*>(out + sl.kp);
-    float* kpn = reinterpret_cast<float*>(out + sl.kpn);
     const int lane = t & 31, warp = t >> 5;
     for (int y = warp; y < rows; y += 32) {
         int pos = y ? base[y - 1] : 0;
@@ -176,10 +159,6 @@ __global__ void __launch_bounds__(1024) lv_fast_compact_kernel(const char* stage
                 const int p = pos + __popc(b & ((1u << lane) - 1));
                 kp[2 * p] = (float)x;
                 kp[2 * p + 1] = (float)y;
-                double X, Y;
-                lift_pinhole(intr.v, (double)x, (double)y, X, Y);
-                kpn[2 * p] = (float)X;
-                kpn[2 * p + 1] = (float)Y;
             }
             pos += __popc(b);
         }
@@ -200,6 +179,27 @@ __global__ void __launch_bounds__(1024) lv_fast_compact_kernel(const char* stage
         h->n_corners = total;
         h->attached = 1;
     }
+}
+
+constexpr int LIFT_THREADS = 128;
+
+// liftProjective / z of the compacted corners (computeBRIEFPoint, keyframe.cpp:108), one thread per corner, stored as float
+// like the reference's cv::Point2f.  A grid over max_corners; nothing to do when the corners overflowed.
+__global__ void __launch_bounds__(LIFT_THREADS) lv_lift_kernel(const char* scratch, char* slot, size_t scratch_stride, size_t slot_stride,
+                                                               int rows, int cols, int max_window, int max_corners, Intr intr,
+                                                               int camera_model, double xi) {
+    const LvSlotLayout sl = lv_slot_layout(max_window, max_corners);
+    const int* status = reinterpret_cast<const int*>(scratch + blockIdx.z * scratch_stride + lv_attach_layout(rows, cols).status);
+    if (status[1]) return;
+    const int p = blockIdx.x * LIFT_THREADS + threadIdx.x;
+    if (p >= status[0]) return;
+    char* out = slot + blockIdx.z * slot_stride;
+    const float* kp = reinterpret_cast<const float*>(out + sl.kp);
+    float* kpn = reinterpret_cast<float*>(out + sl.kpn);
+    double X, Y;
+    lift_projective(camera_model, intr.v, xi, (double)kp[2 * p], (double)kp[2 * p + 1], X, Y);
+    kpn[2 * p] = (float)X;
+    kpn[2 * p + 1] = (float)Y;
 }
 
 // BRIEF (DVision BRIEF::compute on the blurred image): one warp per point; blockIdx.y = 0 window points (staging uv),
@@ -676,11 +676,17 @@ __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char*
 
 }  // namespace
 
+void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s) {
+    Intr in;
+    for (int i = 0; i < 8; i++) in.v[i] = L.intrinsics[i];
+    lv_lift_kernel<<<dim3((L.max_corners + LIFT_THREADS - 1) / LIFT_THREADS, 1, 1), LIFT_THREADS, 0, s>>>(
+        L.scratch, L.slot, lv_attach_layout(L.rows, L.cols).total, lv_slot_layout(L.max_window, L.max_corners).total, L.rows, L.cols,
+        L.max_window, L.max_corners, in, L.camera_model, L.xi);
+}
+
 int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev) {
     const size_t stage_stride = lv_stage_layout(L.rows, L.cols, L.max_window).total, scratch_stride = lv_attach_layout(L.rows, L.cols).total;
     const size_t slot_stride = lv_slot_layout(L.max_window, L.max_corners).total;
-    Intr in;
-    for (int i = 0; i < 8; i++) in.v[i] = L.intrinsics[i];
     if (ev) cudaEventRecord(ev[0], s);
     lv_blur_kernel<<<dim3((L.cols + BLUR_TX - 1) / BLUR_TX, (L.rows + BLUR_TY - 1) / BLUR_TY, 1), dim3(BLUR_TX, BLUR_TY), 0, s>>>(
         L.stage, L.scratch, stage_stride, scratch_stride, L.rows, L.cols);
@@ -688,12 +694,13 @@ int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev) {
     lv_fast_score_kernel<<<dim3((L.cols + 127) / 128, L.rows, 1), 128, 0, s>>>(L.stage, L.scratch, stage_stride, scratch_stride, L.rows, L.cols);
     lv_fast_nms_kernel<<<dim3(1, L.rows, 1), 256, 0, s>>>(L.scratch, scratch_stride, L.rows, L.cols);
     lv_fast_compact_kernel<<<dim3(1, 1, 1), 1024, 0, s>>>(L.stage, L.scratch, L.slot, stage_stride, scratch_stride, slot_stride, L.rows,
-                                                           L.cols, L.max_window, L.max_corners, in);
+                                                           L.cols, L.max_window, L.max_corners);
+    launch_lv_lift(L, s);
     if (ev) cudaEventRecord(ev[2], s);
     lv_brief_kernel<<<dim3(64, 2, 1), 256, 0, s>>>(L.stage, L.scratch, L.slot, stage_stride, scratch_stride, slot_stride, L.pattern, L.rows,
                                                     L.cols, L.max_window, L.max_corners);
     if (ev) cudaEventRecord(ev[3], s);
-    return 5;
+    return 6;
 }
 
 int launch_lv_connect(const LvConnLaunch& L, cudaStream_t s, cudaEvent_t* ev, int match) {

@@ -15,10 +15,15 @@ struct LvAttachLaunch {
     char* slot;
     const int* pattern;  // device, 256 x (x1, y1, x2, y2)
     int rows, cols, max_window, max_corners;
-    double intrinsics[8];  // PINHOLE fx fy cx cy k1 k2 p1 p2
+    double intrinsics[8];  // in the order of camera_model (camera_lift.h)
+    int camera_model;      // CAM_PINHOLE, CAM_MEI or CAM_KANNALA_BRANDT
+    double xi;             // MEI only
 };
-// ev (may be NULL): 4 events recorded before the blur, the FAST stage, BRIEF and after BRIEF.  Returns launches.
+// ev (may be NULL): 4 events recorded before the blur, the FAST stage (FAST, compaction and the corner lift), BRIEF and
+// after BRIEF.  Returns launches.
 int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev);
+// The corner lift alone: the status and the corners kp already in scratch and slot.
+void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s);
 
 // n_jobs verifications.  jobs (device): per job the slot byte offsets of cur and old in the arena (2 x long long).
 // Scratch (lv_conn_layout) and result (lv_result_doubles) per job at the given strides.

@@ -32,6 +32,7 @@
 #include "fm_ransac.h"
 #include "hostpool.h"
 #include "kprof.h"
+#include "camera_lift.h"
 #include "cuda_check.h"
 #include "vinsb200/tracker.h"
 
@@ -212,100 +213,12 @@ std::vector<int> disc_half_widths(int radius) {
     return hw;
 }
 
-// Recursive inverse of the radial-tangential distortion, n = 8 (PinholeCamera.cc:487-503, CataCamera.cc:596-611).
-inline void undistort_radtan(double k1, double k2, double p1, double p2, double mx_d, double my_d, double& ux, double& uy) {
-    ux = mx_d;
-    uy = my_d;
-    for (int i = 0; i < 8; ++i) {
-        const double x2 = ux * ux, y2 = uy * uy, xy = ux * uy, rho2 = x2 + y2;
-        const double rad = k1 * rho2 + k2 * rho2 * rho2;
-        const double ddx = ux * rad + 2.0 * p1 * xy + p2 * (rho2 + 2.0 * x2);
-        const double ddy = uy * rad + 2.0 * p2 * xy + p1 * (rho2 + 2.0 * y2);
-        ux = mx_d - ddx;
-        uy = my_d - ddy;
-    }
-}
-
-// EquidistantCamera::backprojectSymmetric (EquidistantCamera.cc:716-818): the smallest non-negative real root of
-// k5 t^9 + k4 t^7 + k3 t^5 + k2 t^3 + t - r = 0, r itself when there is none.  The reference takes it from the eigenvalues of
-// the companion matrix; here the first sign change of the polynomial on a fine grid is bracketed and polished by
-// bisection + Newton (the same root to rounding).
-double kb_theta(const double kin[4], double r) {
-    // the reference lowers the polynomial degree by 2 for EVERY zero coefficient, whichever it is, and drops the terms above
-    // the resulting degree (EquidistantCamera.cc:733-770)
-    int npow = 9;
-    for (int i = 0; i < 4; i++) npow -= kin[i] == 0.0 ? 2 : 0;
-    if (npow == 1) return r;
-    double k[4];
-    for (int i = 0; i < 4; i++) k[i] = 2 * i + 3 <= npow ? kin[i] : 0.0;
-    auto f = [&](double t) {
-        const double t2 = t * t;
-        return t * (1.0 + t2 * (k[0] + t2 * (k[1] + t2 * (k[2] + t2 * k[3])))) - r;
-    };
-    auto df = [&](double t) {
-        const double t2 = t * t;
-        return 1.0 + t2 * (3.0 * k[0] + t2 * (5.0 * k[1] + t2 * (7.0 * k[2] + t2 * 9.0 * k[3])));
-    };
-    if (r <= 1e-10) return 0.0;  // f(0) = -r: the root is within the reference's tolerance of zero
-    const double step = 1.0 / 512.0;
-    double lo = 0.0;
-    for (int i = 1; i <= 4096; i++) {  // up to theta = 8 rad, far beyond any lens
-        double hi = i * step;
-        if (f(hi) >= 0.0) {
-            for (int it = 0; it < 24; it++) {  // bisection narrows the bracket, Newton finishes
-                const double mid = 0.5 * (lo + hi);
-                if (f(mid) < 0.0) lo = mid; else hi = mid;
-            }
-            double t = 0.5 * (lo + hi);
-            for (int it = 0; it < 20; it++) {
-                const double d = df(t);
-                if (d == 0.0) break;
-                const double tn = t - f(t) / d;
-                if (!(tn >= lo && tn <= hi)) break;
-                if (tn == t) break;
-                t = tn;
-            }
-            return t;
-        }
-        lo = hi;
-    }
-    return r;
-}
-
-// CameraPtr::liftProjective followed by the division by z that every caller applies (feature_tracker.cpp:179-186, 268-272):
-//   PINHOLE  PinholeCamera.cc:450-510      intrinsics = fx fy cx cy k1 k2 p1 p2
-//   MEI      CataCamera.cc:556-625         intrinsics = gamma1 gamma2 u0 v0 k1 k2 p1 p2, cfg.xi
-//   KANNALA_BRANDT  EquidistantCamera.cc:428-442   intrinsics = mu mv u0 v0 k2 k3 k4 k5
+// CameraPtr::liftProjective followed by the division by z that every caller applies (feature_tracker.cpp:179-186, 268-272);
+// camera_lift.h holds the three models.
+static_assert(VT_CAMERA_PINHOLE == vb::CAM_PINHOLE && VT_CAMERA_MEI == vb::CAM_MEI && VT_CAMERA_KANNALA_BRANDT == vb::CAM_KANNALA_BRANDT,
+              "camera model values");
 void lift_projective(const vt_config& c, double px, double py, double& X, double& Y) {
-    const double fx = c.intrinsics[0], fy = c.intrinsics[1], cx = c.intrinsics[2], cy = c.intrinsics[3];
-    const double k1 = c.intrinsics[4], k2 = c.intrinsics[5], p1 = c.intrinsics[6], p2 = c.intrinsics[7];
-    const double mx_d = (1.0 / fx) * px + (-cx / fx), my_d = (1.0 / fy) * py + (-cy / fy);
-    if (c.camera_model == VT_CAMERA_KANNALA_BRANDT) {
-        const double r = std::sqrt(mx_d * mx_d + my_d * my_d);
-        const double phi = r < 1e-10 ? 0.0 : std::atan2(my_d, mx_d);
-        const double theta = kb_theta(&c.intrinsics[4], r);
-        const double Px = std::sin(theta) * std::cos(phi), Py = std::sin(theta) * std::sin(phi), Pz = std::cos(theta);
-        X = Px / Pz;
-        Y = Py / Pz;
-        return;
-    }
-    double ux = mx_d, uy = my_d;
-    if (!(k1 == 0.0 && k2 == 0.0 && p1 == 0.0 && p2 == 0.0)) undistort_radtan(k1, k2, p1, p2, mx_d, my_d, ux, uy);
-    if (c.camera_model == VT_CAMERA_MEI) {
-        const double xi = c.xi;
-        double Pz;
-        if (xi == 1.0)
-            Pz = (1.0 - ux * ux - uy * uy) / 2.0;
-        else {
-            const double rho2 = ux * ux + uy * uy;
-            Pz = 1.0 - xi * (rho2 + 1.0) / (xi + std::sqrt(1.0 + (1.0 - xi * xi) * rho2));
-        }
-        X = ux / Pz;
-        Y = uy / Pz;
-        return;
-    }
-    X = ux;
-    Y = uy;
+    vb::lift_projective(c.camera_model, c.intrinsics, c.xi, px, py, X, Y);
 }
 
 template <class T>

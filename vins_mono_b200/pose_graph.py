@@ -231,6 +231,9 @@ def _bind_loop(lib):
     V = C.c_void_p
     lib.vp_loop_enable.argtypes = [V, C.POINTER(LoopConfig)]
     lib.vp_batch_loop_enable.argtypes = [V, C.POINTER(LoopConfig)]
+    lib.vp_loop_enable_camera.argtypes = [V, C.POINTER(LoopConfig), C.c_int, C.c_double]
+    lib.vp_batch_loop_enable_camera.argtypes = [V, C.POINTER(LoopConfig), C.c_int, C.c_double]
+    lib.vp_debug_lift.argtypes = [C.c_int, V, C.c_double, C.c_int, V, V]
     lib.vp_attach_keyframe.argtypes = [V, C.c_int, V, V, V, C.c_size_t, C.c_int, V, V, V, V, C.POINTER(C.c_int)]
     lib.vp_find_connection.argtypes = [V, C.c_int, C.c_int, C.POINTER(LoopResult), C.c_int, V]
     lib.vp_batch_find_connection.argtypes = [V, V, V, V, C.c_int, V, V]
@@ -259,10 +262,12 @@ def _result(r, lst):
                 old_R=np.array(r.old_R9[:]).reshape(3, 3), old_T=np.array(r.old_T3[:]), points=lst[:r.n_points].copy())
 
 
-def _enable_loop(self, cfg):
+def _enable_loop(self, cfg, camera_model=0, xi=0.0):
+    """camera_model: 0 PINHOLE, 1 MEI (xi = mirror_parameters.xi), 2 KANNALA_BRANDT; cfg.intrinsics in the model's order
+    (config.loop_kwargs reads both from a YAML file)."""
     _bind_loop(self.lib)
     self._loop_cap = cfg.max_window
-    self._check(self.lib.vp_loop_enable(self.h, C.byref(cfg)))
+    self._check(self.lib.vp_loop_enable_camera(self.h, C.byref(cfg), int(camera_model), float(xi)))
 
 
 def _attach_keyframe(self, index, vio_P, vio_Q_wxyz, image, point_3d, point_uv, point_norm, point_id):
@@ -295,12 +300,12 @@ PoseGraph.find_connection = _find_connection
 PoseGraph.loop_timing = _loop_timing
 
 
-def _batch_enable_loop(self, cfg):
+def _batch_enable_loop(self, cfg, camera_model=0, xi=0.0):
     _bind_loop(self.lib)
     self._loop_cap = cfg.max_window
     for m in self.members:
         m._loop_cap = cfg.max_window
-    rc = self.lib.vp_batch_loop_enable(self.h, C.byref(cfg))
+    rc = self.lib.vp_batch_loop_enable_camera(self.h, C.byref(cfg), int(camera_model), float(xi))
     if rc < 0:
         raise PoseGraphError(rc, self.lib.vp_batch_last_error(self.h).decode())
 
@@ -379,3 +384,14 @@ def debug_pnp(point_3d, norm):
     if rc:
         raise RuntimeError(f"vp_debug_pnp failed with status {rc}")
     return Rt[:9].reshape(3, 3), Rt[9:], n_in.value, mask.astype(bool)
+
+
+def debug_lift(camera_model, intrinsics, xi, uv):
+    """The device lift of the key-frame corners (liftProjective / z) of float pixel positions uv (n, 2): (n, 2) float32."""
+    K = _d(intrinsics).reshape(8)
+    pts = np.ascontiguousarray(uv, np.float32).reshape(-1, 2)
+    xy = np.zeros_like(pts)
+    rc = _lib().vp_debug_lift(int(camera_model), _p(K), float(xi), len(pts), _p(pts), _p(xy))
+    if rc:
+        raise RuntimeError(f"vp_debug_lift failed with status {rc}")
+    return xy
