@@ -117,3 +117,18 @@ def test_replay_batch_matches_python_loop():
     ses.close()
     tb.close()
     eb.close()
+
+
+def test_member_keeps_its_batch_alive_and_fails_cleanly_after_close(monkeypatch):
+    import gc
+    from vins_mono_b200 import TrackerBatch, VinsError, load_library
+    cfg = synth.tracker_config_dict(rows=ROWS, cols=COLS, max_cnt=60, min_dist=20)
+    m = TrackerBatch(2, **cfg).members[0]  # the batch itself is never bound to a name
+    gc.collect()
+    assert m.result()["ids"].size == 0 and m.traffic() == (0.0, 0.0)
+    b = TrackerBatch(2, **cfg)
+    m = b.members[1]
+    b.close()
+    monkeypatch.setattr(load_library(), "vt_count", lambda *a: pytest.fail("a closed member reached the library"))
+    with pytest.raises(VinsError):
+        m.result()

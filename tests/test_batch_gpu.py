@@ -120,3 +120,19 @@ def test_batch_of_64_sequences_runs():
     # one launch chain per frame regardless of the batch size: zero + linearize + 8 x 3 + finish + 3 marginalisation + jobs
     assert max(launches) <= batch.groups() * (1 + 8 * 3 + 1 + 4 + 1), launches   # per launch group
     batch.close()
+
+
+def test_member_keeps_its_batch_alive_and_fails_cleanly_after_close(monkeypatch):
+    import gc
+    from vins_mono_b200 import EstimatorBatch, VinsError, load_library
+    m = EstimatorBatch(2, tic=synth.TIC, ric=synth.RIC).members[0]  # the batch itself is never bound to a name
+    gc.collect()
+    m.processIMU(0.005, [0, 0, 9.81], [0, 0, 0])
+    states, _ = m.states()
+    assert states.shape == (11, 16) and m.info()["frame_count"] == 0
+    b = EstimatorBatch(2, tic=synth.TIC, ric=synth.RIC)
+    m = b.members[1]
+    b.close()
+    monkeypatch.setattr(load_library(), "ve_get_states", lambda *a: pytest.fail("a closed member reached the library"))
+    with pytest.raises(VinsError):
+        m.states()

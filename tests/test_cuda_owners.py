@@ -2,6 +2,7 @@
 csrc/cuda_check.h, so create paths that fail half-way and destroy paths release the same things.  The GPU tests read the
 owners' live count (vb_debug_live_cuda_objects) rather than the device's free memory, which other processes change."""
 import ctypes as C
+import gc
 import os
 import re
 
@@ -30,6 +31,7 @@ def test_cuda_resources_are_taken_only_through_the_owning_header():
 
 
 def _live(lib):
+    gc.collect()  # a batch and its members reference each other: release the ones earlier tests dropped without close()
     lib.vb_debug_live_cuda_objects.restype = C.c_longlong
     return lib.vb_debug_live_cuda_objects()
 

@@ -16,7 +16,6 @@ def ransac():
     from vins_mono_b200 import build, load_library
     build.build()
     lib = load_library()
-    lib.vt_debug_fundamental_ransac.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p]
 
     def run(p1, p2, thr=1.0, conf=0.99):
         p1, p2 = np.ascontiguousarray(p1, np.float32), np.ascontiguousarray(p2, np.float32)
@@ -129,7 +128,6 @@ def _lift_all(model, prm, px):
     from harness import synth
     from vins_mono_b200 import load_library
     lib = load_library()
-    lib.vt_debug_lift_projective_model.argtypes = [C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
     K = np.array([prm[k] for k in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2")], np.float64)
     out = np.zeros_like(px)
     assert lib.vt_debug_lift_projective_model(model, K.ctypes.data, float(prm.get("xi", 0.0)), px.ctypes.data, len(px), out.ctypes.data) == 0

@@ -8,17 +8,6 @@ import numpy as np
 from vins_mono_b200 import load_library
 
 
-def _lib():
-    lib = load_library()
-    lib.vr_prop_create.restype = C.c_void_p
-    lib.vr_prop_destroy.argtypes = [C.c_void_p]
-    lib.vr_prop_predict.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.vr_prop_update.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 3
-    lib.vr_format_result_row.argtypes = [C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int]
-    lib.vr_decode_pointcloud.argtypes = [C.c_int] + [C.c_void_p] * 9
-    return lib
-
-
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -35,7 +24,7 @@ def qrot(q, v):
 
 
 def test_predict_and_update_follow_the_node():
-    lib = _lib()
+    lib = load_library()
     rng = np.random.default_rng(1)
     n = 40
     t = 10.0 + 0.005 * np.arange(n)
@@ -76,7 +65,7 @@ def test_predict_and_update_follow_the_node():
 
 
 def test_result_row_format():
-    lib = _lib()
+    lib = load_library()
     buf = C.create_string_buffer(256)
     P, Q, V = np.array([1.234567, -0.000004, 12.5]), np.array([0.7071068, 0.0, -0.7071068, 1e-7]), np.array([0.1, -2.25, 3.999996])
     n = lib.vr_format_result_row(1403636579.763555527, _p(P), _p(Q), _p(V), buf, 256)
@@ -88,7 +77,7 @@ def test_result_row_format():
 
 
 def test_pointcloud_decoding():
-    lib = _lib()
+    lib = load_library()
     n = 5
     xyz = np.array([[0.1, -0.2, 1], [0.3, 0.4, 1], [0, 0, 1], [-0.5, 0.25, 1], [0.01, 0.02, 1]], np.float32)
     idp = np.array([7, 123456, 0, 16777216, 42], np.float32)   # ids travel as float32 channel values (exact up to 2^24)
@@ -104,8 +93,7 @@ def test_pointcloud_decoding():
 
 def test_relo_message_decoding():
     """estimator_node.cpp:273-291: match_points PointCloud -> (match_points, relo_t, relo_r, frame_index)."""
-    lib = _lib()
-    lib.vr_decode_relo_message.argtypes = [C.c_int] + [C.c_void_p] * 6
+    lib = load_library()
     rng = np.random.default_rng(2)
     n = 17
     xyz = np.c_[rng.uniform(-0.5, 0.5, (n, 2)), np.sort(rng.integers(0, 4000, n))].astype(np.float32)

@@ -35,7 +35,6 @@ def test_imu_batches_equal_python_feeder():
     counts = np.zeros(len(stamps), np.int32)
     dt, a, g = np.zeros(cap), np.zeros((cap, 3)), np.zeros((cap, 3))
     p = lambda x: x.ctypes.data_as(C.c_void_p)
-    lib.vr_debug_imu_batches.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 4
     n = lib.vr_debug_imu_batches(len(t_imu), p(t_imu), p(acc), p(gyr), len(stamps), p(stamps), cap, p(counts), p(dt), p(a), p(g))
     assert n == len(want) and counts.tolist() == counts_want
     got = np.c_[dt[:n], a[:n], g[:n]]

@@ -2,7 +2,6 @@
 oracle/camera_models.py and the library's host lift, loop_kwargs against tracker_kwargs / estimator_kwargs on the reference's
 configuration files, the fisheye revisit sequence's project(lift(pixel)) round trip, the new symbols exported and creation
 failing without a GPU.  The fisheye twin is tests/loop_camera_twin.py."""
-import ctypes as C
 import glob
 import os
 import re
@@ -45,7 +44,6 @@ SETS = {s[0]: s for s in camera_sets()}
 def host_lift(model, intr, xi, px):
     from vins_mono_b200 import load_library
     lib = load_library()
-    lib.vt_debug_lift_projective_model.argtypes = [C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
     K, px = np.ascontiguousarray(intr, np.float64), np.ascontiguousarray(px, np.float64)
     out = np.zeros_like(px)
     assert lib.vt_debug_lift_projective_model(model, K.ctypes.data, float(xi), px.ctypes.data, len(px), out.ctypes.data) == 0

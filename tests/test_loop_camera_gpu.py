@@ -139,7 +139,7 @@ def test_attach_and_verification_agree_with_the_twin(name):
             assert ulps(r["points"][:, :2].astype(np.float32), ko.kp_norm[idx]).max() <= (0 if kw["camera_model"] == 1 else 1)
 
 
-def test_pinhole_through_the_camera_entry_equals_vp_loop_enable():
+def test_pinhole_camera_entry_equals_vp_loop_enable():
     from vins_mono_b200 import pose_graph as pg
     seq = synth.Sequence(seed=0, duration=12.0)
     pts = loop_revisit.corner_landmarks(seq, np.arange(0.2, 12.0, 0.5))
@@ -150,7 +150,6 @@ def test_pinhole_through_the_camera_entry_equals_vp_loop_enable():
         g = pg.PoseGraph(max_keyframes=4)
         cfg = _loop_cfg(kw)
         if entry == "vp_loop_enable":
-            pg._bind_loop(g.lib)
             g._loop_cap = cfg.max_window
             assert g.lib.vp_loop_enable(g.h, C.byref(cfg)) == 0
         else:

@@ -36,8 +36,6 @@ def test_out_of_range_anchor_capacity_is_invalid(max_anchors):
     from vins_mono_b200.pose_graph import PoseGraphConfig
     build.build()
     lib = load_library()
-    lib.vp_create.argtypes = [ctypes.POINTER(PoseGraphConfig), ctypes.POINTER(ctypes.c_void_p)]
-    lib.vp_batch_create.argtypes = [ctypes.POINTER(PoseGraphConfig), ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]
     cfg = PoseGraphConfig(max_keyframes=64, fast_relocalization=0, device=0, max_anchors=max_anchors)
     h = ctypes.c_void_p()
     assert lib.vp_create(ctypes.byref(cfg), ctypes.byref(h)) == -1 and not h.value

@@ -314,3 +314,19 @@ def test_later_optimisation_uses_the_updated_loop_info():
     _, P_upd, _, _ = g.path()
     _, P_old, _, _ = run(True, False).path()
     assert np.abs(P_upd - P_old).max() > 1e-3  # the replaced measurement changed the later solve
+
+
+def test_member_keeps_its_batch_alive_and_fails_cleanly_after_close(monkeypatch):
+    import gc
+    from vins_mono_b200 import VinsError, load_library
+    _, PoseGraphBatch, _, _ = _vp()
+    g = PoseGraphBatch(2, max_keyframes=8)[0]  # the batch itself is never bound to a name
+    gc.collect()
+    g.add_keyframe(0.0, [1, 2, 3], [1, 0, 0, 0])
+    assert g.info()["keyframes"] == 1 and np.array_equal(g.path()[1], [[1, 2, 3]])
+    b = PoseGraphBatch(2, max_keyframes=8)
+    m = b[1]
+    b.close()
+    monkeypatch.setattr(load_library(), "vp_info", lambda *a: pytest.fail("a closed member reached the library"))
+    with pytest.raises(VinsError):
+        m.info()

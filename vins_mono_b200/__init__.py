@@ -4,6 +4,7 @@ The product is lib/libvinsb200.so (hand-written CUDA for sm_90a + host glue); th
 ctypes mirror of the reference's host classes for tests and benchmarks.  There is no CPU fallback:
 loading fails loudly when the library is missing, creating a tracker fails when no CUDA device exists.
 """
+from ._abi import VinsError  # noqa: F401
 from .tracker import FeatureTracker, TrackerBatch, TrackerConfig, load_library, LIB_PATH  # noqa: F401
 from .estimator import Estimator, EstimatorBatch, EstimatorConfig, debug_projection_factor, debug_imu_factor  # noqa: F401
 from .replay import ReplaySession  # noqa: F401

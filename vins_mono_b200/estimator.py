@@ -6,80 +6,7 @@ import ctypes as C
 
 import numpy as np
 
-from .tracker import load_library
-
-
-class EstimatorConfig(C.Structure):
-    _fields_ = [("window_size", C.c_int), ("max_features", C.c_int), ("num_iterations", C.c_int),
-                ("estimate_extrinsic", C.c_int), ("estimate_td", C.c_int), ("focal_length", C.c_double),
-                ("keyframe_parallax", C.c_double), ("acc_n", C.c_double), ("gyr_n", C.c_double), ("acc_w", C.c_double),
-                ("gyr_w", C.c_double), ("g_norm", C.c_double), ("init_depth", C.c_double), ("td", C.c_double),
-                ("tr", C.c_double), ("row", C.c_double), ("tic", C.c_double * 3), ("ric", C.c_double * 9),
-                ("device", C.c_int)]
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
-
-
-def _d(a):
-    return np.ascontiguousarray(a, np.float64)
-
-
-_bound = False
-
-
-def _bind(lib):
-    global _bound
-    if _bound:
-        return
-    lib.ve_last_error.restype = C.c_char_p
-    lib.ve_last_error.argtypes = [C.c_void_p]
-    lib.ve_create.argtypes = [C.POINTER(EstimatorConfig), C.POINTER(C.c_void_p)]
-    lib.ve_destroy.argtypes = [C.c_void_p]
-    lib.ve_clear_state.argtypes = [C.c_void_p]
-    lib.ve_set_seed.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_process_imu.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]
-    lib.ve_process_image.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double]
-    lib.ve_get_states.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
-    lib.ve_info.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_get_prior.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
-    lib.ve_last_timing.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    lib.ve_solver_debug.argtypes = [C.c_void_p, C.c_void_p]
-    lib.ve_process_imu_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_set_profile.argtypes = [C.c_void_p, C.c_int]
-    lib.ve_kernel_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_last_traffic.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    lib.ve_get_extrinsic.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_batch_create.argtypes = [C.POINTER(EstimatorConfig), C.c_int, C.POINTER(C.c_void_p)]
-    lib.ve_batch_destroy.argtypes = [C.c_void_p]
-    lib.ve_batch_size.argtypes = [C.c_void_p]
-    lib.ve_batch_groups.argtypes = [C.c_void_p]
-    lib.ve_batch_member.argtypes = [C.c_void_p, C.c_int]
-    lib.ve_batch_member.restype = C.c_void_p
-    lib.ve_batch_last_error.argtypes = [C.c_void_p]
-    lib.ve_batch_last_error.restype = C.c_char_p
-    lib.ve_batch_process_image.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_batch_last_timing.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    lib.ve_batch_set_profile.argtypes = [C.c_void_p, C.c_int]
-    lib.ve_batch_kernel_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_batch_sync.argtypes = [C.c_void_p]
-    lib.ve_debug_projection_factor.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.c_void_p]
-    lib.ve_debug_imu_factor.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_init_info.argtypes = [C.c_void_p, C.c_void_p]
-    lib.ve_debug_ex_rotation.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_set_relo_frame.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.ve_get_relocalization.argtypes = [C.c_void_p, C.c_void_p]
-    lib.ve_get_headers.argtypes = [C.c_void_p, C.c_void_p]
-    lib.ve_debug_relative_rt.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    lib.ve_debug_solve_pnp.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.ve_debug_sfm_construct.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_double] + \
-        [C.c_void_p] * 2 + \
-        [C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double)]
-    lib.ve_debug_initial_structure.argtypes = [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 7 + [C.c_int] + [C.c_void_p] * 6 + \
-        [C.c_double, C.c_double] + [C.c_void_p] * 6 + [C.POINTER(C.c_double)]
-    _bound = True
+from ._abi import Batch, EstimatorConfig, Handle, check, f64, load_library, ptr
 
 
 def _make_config(window_size=10, max_features=1000, num_iterations=8, estimate_extrinsic=0, estimate_td=0,
@@ -94,56 +21,37 @@ def _make_config(window_size=10, max_features=1000, num_iterations=8, estimate_e
     return cfg
 
 
-class Estimator:
+class Estimator(Handle):
     """Drop-in for the reference Estimator: processIMU / processImage, then read Ps, Rs, Vs, Bas, Bgs."""
+    _destroy, _last_error = "ve_destroy", "ve_last_error"
 
     def __init__(self, **kw):
-        self.lib = load_library()
-        _bind(self.lib)
         cfg = _make_config(**kw)
         self.cfg, self.W = cfg, cfg.window_size
-        h = C.c_void_p()
-        rc = self.lib.ve_create(C.byref(cfg), C.byref(h))
-        if rc != 0:
-            raise RuntimeError(f"ve_create failed with status {rc} (-2 = no CUDA device; this library has no CPU path)")
-        self.h = h
-        self._borrowed = False
+        self._open("ve_create", C.byref(cfg))
 
     @classmethod
-    def _member(cls, lib, handle, cfg):
+    def _member(cls, batch, k):
         """Borrowed handle of a batch member (driven and destroyed through its EstimatorBatch)."""
-        self = cls.__new__(cls)
-        self.lib, self.cfg, self.W, self.h, self._borrowed = lib, cfg, cfg.window_size, C.c_void_p(handle), True
+        self = cls._borrow(batch, batch.lib.ve_batch_member(batch.h, k))
+        self.cfg, self.W = batch.cfg, batch.cfg.window_size
         return self
-
-    def close(self):
-        if getattr(self, "h", None):
-            if not self._borrowed:
-                self.lib.ve_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _check(self, rc):
-        if rc < 0:
-            raise RuntimeError(f"vinsb200 error {rc}: {self.lib.ve_last_error(self.h).decode()}")
-        return rc
 
     def setReloFrame(self, frame_stamp, frame_index, match_points, relo_t, relo_r):
         """Estimator::setReloFrame (estimator.h:36): match_points = n x (x, y, feature id).  True when the stamp is in the window."""
-        mp = _d(match_points).reshape(-1, 3)
-        return bool(self._check(self.lib.ve_set_relo_frame(self.h, float(frame_stamp), int(frame_index), len(mp), _p(mp), _p(_d(relo_t)),
-                                                           _p(_d(relo_r).reshape(9)))))
+        mp = f64(match_points).reshape(-1, 3)
+        return bool(self._check(self.lib.ve_set_relo_frame(self.h, float(frame_stamp), int(frame_index), len(mp), ptr(mp), ptr(f64(relo_t)),
+                                                           ptr(f64(relo_r).reshape(9)))))
 
     def headers(self):
         """Stamps of the window frames (Headers[0 .. WINDOW_SIZE])."""
         h = np.zeros(self.W + 1)
-        self._check(self.lib.ve_get_headers(self.h, _p(h)))
+        self._check(self.lib.ve_get_headers(self.h, ptr(h)))
         return h
 
     def relo(self):
         o = np.zeros(24)
-        self._check(self.lib.ve_get_relocalization(self.h, _p(o)))
+        self._check(self.lib.ve_get_relocalization(self.h, ptr(o)))
         return dict(drift_correct_r=o[0:9].reshape(3, 3).copy(), drift_correct_t=o[9:12].copy(), relo_relative_t=o[12:15].copy(),
                     relo_relative_q=o[15:19].copy(), relo_relative_yaw=float(o[19]), pending=bool(o[20]), local_index=int(o[21]),
                     factors=int(o[22]), solves=int(o[23]))
@@ -151,7 +59,7 @@ class Estimator:
     def init_info(self):
         """How the window was initialised: own initialStructure (self_initialised) or a caller-supplied seed."""
         r = np.zeros(8)
-        rc = self._check(self.lib.ve_init_info(self.h, _p(r)))
+        rc = self._check(self.lib.ve_init_info(self.h, ptr(r)))
         return dict(self_initialised=bool(rc), l=int(r[0]), scale=float(r[1]), g=r[2:5].copy(), bundle_iterations=int(r[5]),
                     bundle_cost=float(r[6]), failed_attempts=int(r[7]))
 
@@ -159,26 +67,26 @@ class Estimator:
         self._check(self.lib.ve_clear_state(self.h))
 
     def set_seed(self, rows, ba, bg):
-        rows, ba, bg = _d(rows), _d(ba), _d(bg)
-        self._check(self.lib.ve_set_seed(self.h, len(rows), _p(rows), _p(ba), _p(bg)))
+        rows, ba, bg = f64(rows), f64(ba), f64(bg)
+        self._check(self.lib.ve_set_seed(self.h, len(rows), ptr(rows), ptr(ba), ptr(bg)))
 
     def processIMU(self, dt, linear_acceleration, angular_velocity):
-        a, g = _d(linear_acceleration), _d(angular_velocity)
-        self._check(self.lib.ve_process_imu(self.h, float(dt), _p(a), _p(g)))
+        a, g = f64(linear_acceleration), f64(angular_velocity)
+        self._check(self.lib.ve_process_imu(self.h, float(dt), ptr(a), ptr(g)))
 
     def processImage(self, ids, xyz_uv_vel, stamp):
         ids = np.ascontiguousarray(ids, np.int32)
-        d = _d(xyz_uv_vel)
-        self._check(self.lib.ve_process_image(self.h, len(ids), _p(ids), _p(d), float(stamp)))
+        d = f64(xyz_uv_vel)
+        self._check(self.lib.ve_process_image(self.h, len(ids), ptr(ids), ptr(d), float(stamp)))
 
     def states(self):
         out, td = np.zeros((self.W + 1, 16)), C.c_double(0)
-        self._check(self.lib.ve_get_states(self.h, _p(out), C.byref(td)))
+        self._check(self.lib.ve_get_states(self.h, ptr(out), C.byref(td)))
         return out, td.value
 
     def info(self):
         o, c = np.zeros(10, np.int32), np.zeros(2)
-        self._check(self.lib.ve_info(self.h, _p(o), _p(c)))
+        self._check(self.lib.ve_info(self.h, ptr(o), ptr(c)))
         keys = ["solver_flag", "frame_count", "marginalization_flag", "n_solves", "n_reboots", "landmarks", "visual",
                 "iterations", "successful_steps", "termination"]
         d = {k: int(v) for k, v in zip(keys, o)}
@@ -188,73 +96,59 @@ class Estimator:
     def prior(self, cap=256):
         A, b = np.zeros(cap * cap), np.zeros(cap)
         nb, blk = C.c_int(0), np.zeros(4 * 64, np.int32)
-        n = self._check(self.lib.ve_get_prior(self.h, cap, _p(A), _p(b), C.byref(nb), _p(blk)))
+        n = self._check(self.lib.ve_get_prior(self.h, cap, ptr(A), ptr(b), C.byref(nb), ptr(blk)))
         return A[: n * n].reshape(n, n).copy(), b[:n].copy(), [tuple(int(v) for v in blk[4 * k:4 * k + 4]) for k in range(nb.value)]
 
     KERNELS = ["ba_eval", "ba_reduce", "ba_step", "unused", "marg_build", "marg_solve", "preint_jobs", "ba_finish"]
 
     def processIMU_batch(self, dt, acc, gyr):
-        dt, acc, gyr = _d(dt), _d(acc), _d(gyr)
-        self._check(self.lib.ve_process_imu_batch(self.h, len(dt), _p(dt), _p(acc), _p(gyr)))
+        dt, acc, gyr = f64(dt), f64(acc), f64(gyr)
+        self._check(self.lib.ve_process_imu_batch(self.h, len(dt), ptr(dt), ptr(acc), ptr(gyr)))
 
     def set_profile(self, on):
-        self.lib.ve_set_profile(self.h, int(on))
+        self._check(self.lib.ve_set_profile(self.h, int(on)))
 
     def kernel_times(self):
         ms, cnt = np.zeros(8), np.zeros(8, np.int32)
-        self.lib.ve_kernel_times(self.h, _p(ms), _p(cnt))
+        self._check(self.lib.ve_kernel_times(self.h, ptr(ms), ptr(cnt)))
         return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNELS)}
 
     def traffic(self):
         a, b = C.c_double(0), C.c_double(0)
-        self.lib.ve_last_traffic(self.h, C.byref(a), C.byref(b))
+        self._check(self.lib.ve_last_traffic(self.h, C.byref(a), C.byref(b)))
         return a.value, b.value
 
     def solver_debug(self):
         out = np.zeros(18)
-        self.lib.ve_solver_debug(self.h, _p(out))
+        self._check(self.lib.ve_solver_debug(self.h, ptr(out)))
         return dict(retries=int(out[0]), mu=out[1], radius=out[2], clk=out[3:].astype(np.int64).tolist(), floor_pairs=int(out[12]))
 
     def launch_count(self):
         """Kernel launches of the last processImage (does not wait for a pending marginalisation)."""
         k = C.c_int(0)
-        self.lib.ve_last_timing(self.h, None, C.byref(k))
+        self._check(self.lib.ve_last_timing(self.h, None, C.byref(k)))
         return k.value
 
     def timing(self):
         ms, k = np.zeros(4, np.float32), C.c_int(0)
-        self.lib.ve_last_timing(self.h, _p(ms), C.byref(k))
+        self._check(self.lib.ve_last_timing(self.h, ptr(ms), C.byref(k)))
         return dict(preint_ms=float(ms[0]), solve_ms=float(ms[1]), marg_ms=float(ms[2]), total_ms=float(ms[3]), launches=k.value)
 
     def extrinsic(self):
         t, r = np.zeros(3), np.zeros(9)
-        self._check(self.lib.ve_get_extrinsic(self.h, _p(t), _p(r)))
+        self._check(self.lib.ve_get_extrinsic(self.h, ptr(t), ptr(r)))
         return t, r.reshape(3, 3)
 
 
-class EstimatorBatch:
+class EstimatorBatch(Batch):
     """n independent estimators advancing together (include/vinsb200/estimator.h, ve_batch_*): one launch chain per frame
     for the whole batch.  members[k] is an Estimator mirror for the per-sequence calls (set_seed, processIMU, states ...)."""
+    _destroy, _last_error = "ve_batch_destroy", "ve_batch_last_error"
 
     def __init__(self, n, **kw):
-        self.lib = load_library()
-        _bind(self.lib)
         self.cfg, self.n = _make_config(**kw), n
-        h = C.c_void_p()
-        rc = self.lib.ve_batch_create(C.byref(self.cfg), n, C.byref(h))
-        if rc != 0:
-            raise RuntimeError(f"ve_batch_create failed with status {rc} (-2 = no CUDA device; this library has no CPU path)")
-        self.h = h
-        self.members = [Estimator._member(self.lib, self.lib.ve_batch_member(h, k), self.cfg) for k in range(n)]
-
-    def close(self):
-        if getattr(self, "h", None):
-            for m in self.members:
-                m.h = None
-            self.lib.ve_batch_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        self._open("ve_batch_create", C.byref(self.cfg), n)
+        self.members = [Estimator._member(self, k) for k in range(n)]
 
     def processImage(self, msgs):
         """msgs[k] = (ids, xyz_uv_vel, stamp) or None (member k idles this frame).  Returns the per-member status list."""
@@ -266,66 +160,59 @@ class EstimatorBatch:
         for k, m in enumerate(msgs):
             if m is None:
                 continue
-            ids, d = np.ascontiguousarray(m[0], np.int32), _d(m[1])
+            ids, d = np.ascontiguousarray(m[0], np.int32), f64(m[1])
             keep += [ids, d]
             active[k], cnt[k], stamps[k] = 1, len(ids), float(m[2])
             idp[k], obp[k] = ids.ctypes.data, d.ctypes.data
         status = np.zeros(n, np.int32)
-        rc = self.lib.ve_batch_process_image(self.h, _p(active), _p(cnt), idp, obp, _p(stamps), _p(status))
-        if rc < 0:
-            raise RuntimeError(f"vinsb200 batch error {rc}: {self.lib.ve_batch_last_error(self.h).decode()}")
+        self._check(self.lib.ve_batch_process_image(self.h, ptr(active), ptr(cnt), idp, obp, ptr(stamps), ptr(status)))
         return status
 
     def timing(self):
         ms, k = np.zeros(4, np.float32), C.c_int(0)
-        self.lib.ve_batch_last_timing(self.h, _p(ms), C.byref(k))
+        self._check(self.lib.ve_batch_last_timing(self.h, ptr(ms), C.byref(k)))
         return dict(preint_ms=float(ms[0]), solve_ms=float(ms[1]), marg_ms=float(ms[2]), total_ms=float(ms[3]), launches=k.value)
 
     def launch_count(self):
         k = C.c_int(0)
-        self.lib.ve_batch_last_timing(self.h, None, C.byref(k))
+        self._check(self.lib.ve_batch_last_timing(self.h, None, C.byref(k)))
         return k.value
 
     def groups(self):
-        return int(self.lib.ve_batch_groups(self.h))
+        return self._check(self.lib.ve_batch_groups(self.h))
 
     def set_profile(self, on):
-        self.lib.ve_batch_set_profile(self.h, int(on))
+        self._check(self.lib.ve_batch_set_profile(self.h, int(on)))
 
     def kernel_times(self):
         ms, cnt = np.zeros(8), np.zeros(8, np.int32)
-        self.lib.ve_batch_kernel_times(self.h, _p(ms), _p(cnt))
+        self._check(self.lib.ve_batch_kernel_times(self.h, ptr(ms), ptr(cnt)))
         return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(Estimator.KERNELS)}
 
     def sync(self):
-        self.lib.ve_batch_sync(self.h)
+        self._check(self.lib.ve_batch_sync(self.h))
 
 
 def debug_projection_factor(params23, data12, use_td=False, focal_length=460.0, tr=0.0, row=480.0, robust=False):
     """Residual (2), Jacobian (2 x 20: pose_i 6, pose_j 6, ex 6, depth, td) and rho/2 of one visual factor, evaluated by the
     device code of the solve."""
     lib = load_library()
-    _bind(lib)
-    prm, dat, out = _d(params23), _d(data12), np.zeros(43)
+    prm, dat, out = f64(params23), f64(data12), np.zeros(43)
     assert prm.size == 23 and dat.size == 12
-    rc = lib.ve_debug_projection_factor(_p(prm), _p(dat), int(use_td), float(focal_length), float(tr), float(row), int(robust), _p(out))
-    if rc != 0:
-        raise RuntimeError(f"ve_debug_projection_factor: {rc}")
+    check(lib.ve_debug_projection_factor(ptr(prm), ptr(dat), int(use_td), float(focal_length), float(tr), float(row), int(robust),
+                                         ptr(out)), "ve_debug_projection_factor")
     return out[0:2].copy(), out[2:42].reshape(2, 20).copy(), float(out[42])
 
 
 def debug_imu_factor(ba, bg, dt, acc, gyr, params32=None, noise=(0.08, 0.004, 0.00004, 2.0e-6), g_norm=9.81007):
     """Device pre-integration of the samples (sample 0 seeds acc_0 / gyr_0) and, with params32, the whitened IMU factor."""
     lib = load_library()
-    _bind(lib)
-    dt, acc, gyr = _d(dt), _d(acc), _d(gyr)
+    dt, acc, gyr = f64(dt), f64(acc), f64(gyr)
     pre, fac = np.zeros(686), np.zeros(465)
-    prm = _d(params32) if params32 is not None else None
-    noise = _d(noise)
-    rc = lib.ve_debug_imu_factor(_p(noise), float(g_norm), _p(_d(ba)), _p(_d(bg)), len(dt), _p(dt), _p(acc), _p(gyr), _p(prm), _p(pre),
-                                 _p(fac) if prm is not None else None)
-    if rc != 0:
-        raise RuntimeError(f"ve_debug_imu_factor: {rc}")
+    prm = f64(params32) if params32 is not None else None
+    noise = f64(noise)
+    check(lib.ve_debug_imu_factor(ptr(noise), float(g_norm), ptr(f64(ba)), ptr(f64(bg)), len(dt), ptr(dt), ptr(acc), ptr(gyr), ptr(prm),
+                                  ptr(pre), ptr(fac) if prm is not None else None), "ve_debug_imu_factor")
     out = dict(sum_dt=pre[0], dp=pre[1:4].copy(), dq=pre[4:8].copy(), dv=pre[8:11].copy(), jacobian=pre[11:236].reshape(15, 15).copy(),
                covariance=pre[236:461].reshape(15, 15).copy(), sqrt_info=pre[461:686].reshape(15, 15).copy())
     if prm is not None:
@@ -338,31 +225,25 @@ def _tracks_flat(tracks):
     ids = np.array([t[0] for t in tracks], np.int32)
     start = np.array([t[1] for t in tracks], np.int32)
     nobs = np.array([len(np.asarray(t[2]).reshape(-1, 2)) for t in tracks], np.int32)
-    xy = _d(np.concatenate([np.asarray(t[2], float).reshape(-1, 2) for t in tracks])) if len(tracks) else np.zeros((0, 2))
+    xy = f64(np.concatenate([np.asarray(t[2], float).reshape(-1, 2) for t in tracks])) if len(tracks) else np.zeros((0, 2))
     return ids, start, nobs, xy
 
 
 def debug_relative_rt(corres):
     """MotionEstimator::solveRelativeRT on n x (x0 y0 x1 y1): (ok, Rotation, Translation, inlier_cnt)."""
     lib = load_library()
-    _bind(lib)
-    c = _d(corres).reshape(-1, 4)
+    c = f64(corres).reshape(-1, 4)
     R, T, cnt = np.zeros(9), np.zeros(3), C.c_int()
-    rc = lib.ve_debug_relative_rt(_p(c), len(c), _p(R), _p(T), C.byref(cnt))
-    if rc < 0:
-        raise RuntimeError(f"ve_debug_relative_rt: {rc}")
+    rc = check(lib.ve_debug_relative_rt(ptr(c), len(c), ptr(R), ptr(T), C.byref(cnt)), "ve_debug_relative_rt")
     return bool(rc), R.reshape(3, 3), T, cnt.value
 
 
 def debug_solve_pnp(pts3, pts2, R_initial, P_initial):
     """cv::solvePnP(..., useExtrinsicGuess=true) from (R_initial, P_initial) (world -> camera): (ok, R, t)."""
     lib = load_library()
-    _bind(lib)
-    p3, p2 = _d(pts3).reshape(-1, 3), _d(pts2).reshape(-1, 2)
-    R, t = _d(R_initial).reshape(9).copy(), _d(P_initial).reshape(3).copy()
-    rc = lib.ve_debug_solve_pnp(_p(p3), _p(p2), len(p2), _p(R), _p(t))
-    if rc < 0:
-        raise RuntimeError(f"ve_debug_solve_pnp: {rc}")
+    p3, p2 = f64(pts3).reshape(-1, 3), f64(pts2).reshape(-1, 2)
+    R, t = f64(R_initial).reshape(9).copy(), f64(P_initial).reshape(3).copy()
+    rc = check(lib.ve_debug_solve_pnp(ptr(p3), ptr(p2), len(p2), ptr(R), ptr(t)), "ve_debug_solve_pnp")
     return bool(rc), R.reshape(3, 3), t
 
 
@@ -370,17 +251,14 @@ def debug_sfm_construct(frame_num, l, relative_R, relative_T, tracks, function_t
     """GlobalSFM::construct; tracks = [(id, start_frame, xy[nobs, 2])].  Returns dict(ok, q[F,4] wxyz, T[F,3], points{id: xyz},
     iterations, cost)."""
     lib = load_library()
-    _bind(lib)
     ids, start, nobs, xy = _tracks_flat(tracks)
     q, T = np.zeros((frame_num, 4)), np.zeros((frame_num, 3))
     n_pts, it, cost = C.c_int(), C.c_int(), C.c_double()
     pid, pts = np.zeros(max(len(ids), 1), np.int32), np.zeros((max(len(ids), 1), 3))
-    rR, rT = _d(relative_R).reshape(9), _d(relative_T).reshape(3)
-    rc = lib.ve_debug_sfm_construct(frame_num, l, _p(rR), _p(rT), len(ids), _p(ids), _p(start), _p(nobs), _p(xy),
-                                    float(function_tolerance), _p(q), _p(T), C.byref(n_pts), _p(pid), _p(pts), C.byref(it),
-                                    C.byref(cost))
-    if rc < 0:
-        raise RuntimeError(f"ve_debug_sfm_construct: {rc}")
+    rR, rT = f64(relative_R).reshape(9), f64(relative_T).reshape(3)
+    rc = check(lib.ve_debug_sfm_construct(frame_num, l, ptr(rR), ptr(rT), len(ids), ptr(ids), ptr(start), ptr(nobs), ptr(xy),
+                                          float(function_tolerance), ptr(q), ptr(T), C.byref(n_pts), ptr(pid), ptr(pts), C.byref(it),
+                                          C.byref(cost)), "ve_debug_sfm_construct")
     return dict(ok=bool(rc), q=q, T=T, points={int(pid[k]): pts[k].copy() for k in range(n_pts.value)}, iterations=it.value,
                 cost=cost.value)
 
@@ -390,28 +268,25 @@ def debug_initial_structure(headers, frames, tracks, ric, tic, g_norm=9.81007, f
     image (imu / lin of frame 0 unused); tracks = [(id, start_frame, xy[nobs,2])].  Returns dict(code, l, R[n,3,3], T[n,3], x, g,
     delta_bg, bundle_iterations, bundle_cost, key_frames)."""
     lib = load_library()
-    _bind(lib)
-    hd = _d(headers)
+    hd = f64(headers)
     na = len(frames)
-    stamps = _d([f["t"] for f in frames])
+    stamps = f64([f["t"] for f in frames])
     pts_off = np.zeros(na + 1, np.int32)
     pts_off[1:] = np.cumsum([len(f["ids"]) for f in frames])
     pt_ids = np.ascontiguousarray(np.concatenate([np.asarray(f["ids"], np.int32) for f in frames]), np.int32)
-    pt_xy = _d(np.concatenate([np.asarray(f["xy"], float).reshape(-1, 2) for f in frames]))
+    pt_xy = f64(np.concatenate([np.asarray(f["xy"], float).reshape(-1, 2) for f in frames]))
     imu_off = np.zeros(na + 1, np.int32)
     imu_off[1:] = np.cumsum([0 if k == 0 else len(f["imu"]) for k, f in enumerate(frames)])
     rows = [np.asarray(f["imu"], float).reshape(-1, 7) for k, f in enumerate(frames) if k > 0]
-    imu7 = _d(np.concatenate(rows)) if rows else np.zeros((0, 7))
-    lin6 = _d([np.zeros(6) if k == 0 else np.asarray(f["lin"], float) for k, f in enumerate(frames)])
+    imu7 = f64(np.concatenate(rows)) if rows else np.zeros((0, 7))
+    lin6 = f64([np.zeros(6) if k == 0 else np.asarray(f["lin"], float) for k, f in enumerate(frames)])
     ids, start, nobs, xy = _tracks_flat(tracks)
     fR, fT, x = np.zeros((na, 9)), np.zeros((na, 3)), np.zeros(3 * na + 3)
     g3, dbg, info, cost = np.zeros(3), np.zeros(3), np.zeros(4, np.int32), C.c_double()
-    rc = lib.ve_debug_initial_structure(len(hd), _p(hd), na, _p(stamps), _p(pts_off), _p(pt_ids), _p(pt_xy), _p(imu_off), _p(imu7),
-                                        _p(lin6), len(ids), _p(ids), _p(start), _p(nobs), _p(xy), _p(_d(ric).reshape(9)),
-                                        _p(_d(tic).reshape(3)), float(g_norm), float(function_tolerance), _p(fR), _p(fT), _p(x), _p(g3), _p(dbg), _p(info),
-                                        C.byref(cost))
-    if rc < 0:
-        raise RuntimeError(f"ve_debug_initial_structure: {rc}")
+    rc = check(lib.ve_debug_initial_structure(len(hd), ptr(hd), na, ptr(stamps), ptr(pts_off), ptr(pt_ids), ptr(pt_xy), ptr(imu_off),
+                                              ptr(imu7), ptr(lin6), len(ids), ptr(ids), ptr(start), ptr(nobs), ptr(xy), ptr(f64(ric).reshape(9)),
+                                              ptr(f64(tic).reshape(3)), float(g_norm), float(function_tolerance), ptr(fR), ptr(fT), ptr(x),
+                                              ptr(g3), ptr(dbg), ptr(info), C.byref(cost)), "ve_debug_initial_structure")
     return dict(code=rc, l=int(info[0]), R=fR.reshape(na, 3, 3), T=fT, x=x, g=g3, delta_bg=dbg, bundle_iterations=int(info[1]),
                 bundle_cost=cost.value, key_frames=int(info[2]))
 
@@ -419,15 +294,12 @@ def debug_initial_structure(headers, frames, tracks, ric, tic, g_norm=9.81007, f
 def debug_ex_rotation(corres_list, dq_list, window_size=10, rc_given=None):
     """InitialEXRotation::CalibrationExRotation called once per (corres[n,4], delta_q wxyz) pair: (ric[k,3,3], ok[k], cov[k], Rc[k,3,3] = the camera rotations solveRelativeR found)."""
     lib = load_library()
-    _bind(lib)
     n = len(corres_list)
     off = np.zeros(n + 1, np.int32)
     off[1:] = np.cumsum([len(np.asarray(c).reshape(-1, 4)) for c in corres_list])
-    c4 = _d(np.concatenate([np.asarray(c, float).reshape(-1, 4) for c in corres_list])) if n else np.zeros((0, 4))
-    dq = _d(dq_list).reshape(-1, 4)
+    c4 = f64(np.concatenate([np.asarray(c, float).reshape(-1, 4) for c in corres_list])) if n else np.zeros((0, 4))
+    dq = f64(dq_list).reshape(-1, 4)
     ric, ok, cov, rcam = np.zeros((n, 9)), np.zeros(n, np.int32), np.zeros(n), np.zeros((n, 9))
-    rc = lib.ve_debug_ex_rotation(n, _p(off), _p(c4), _p(dq), int(window_size), _p(ric), _p(ok), _p(cov), _p(rcam),
-                                  _p(_d(rc_given).reshape(-1, 9)) if rc_given is not None else None)
-    if rc < 0:
-        raise RuntimeError(f"ve_debug_ex_rotation: {rc}")
+    check(lib.ve_debug_ex_rotation(n, ptr(off), ptr(c4), ptr(dq), int(window_size), ptr(ric), ptr(ok), ptr(cov), ptr(rcam),
+                                   ptr(f64(rc_given).reshape(-1, 9)) if rc_given is not None else None), "ve_debug_ex_rotation")
     return ric.reshape(n, 3, 3), ok.astype(bool), cov, rcam.reshape(n, 3, 3)

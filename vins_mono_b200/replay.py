@@ -7,37 +7,22 @@ import ctypes as C
 
 import numpy as np
 
-from .tracker import load_library
+from ._abi import Handle, ReplaySequence, f64, ptr
 
 
-class _Seq(C.Structure):
-    _fields_ = [("images", C.c_void_p), ("row_stride", C.c_size_t), ("frame_stride", C.c_size_t), ("n_images", C.c_int),
-                ("images_on_device", C.c_int), ("stamps", C.c_void_p), ("n_imu", C.c_int), ("imu_t", C.c_void_p),
-                ("acc", C.c_void_p), ("gyr", C.c_void_p)]
-
-
-class ReplaySession:
+class ReplaySession(Handle):
     """sequences: list of dicts(images=<numpy u8 [n,h,w] | int device pointer>, shape=(n,h,w) when a pointer is given,
     stamps, imu_t, acc, gyr).  trackers / estimators: the Python mirrors (their .h handles are borrowed)."""
+    _destroy, _last_error = "vr_close", "vr_last_error"
 
     def __init__(self, trackers, estimators, sequences):
         """trackers / estimators: lists of FeatureTracker / Estimator mirrors (one thread pair per sequence), or a TrackerBatch
         and an EstimatorBatch (batch mode: one tracker loop and one estimator loop, one launch chain per step for all)."""
-        self.lib = load_library()
-        L = self.lib
         batch_mode = not isinstance(trackers, (list, tuple))
-        L.vr_open_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.vr_open.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.vr_advance.argtypes = [C.c_void_p, C.c_int]
-        L.vr_close.argtypes = [C.c_void_p]
-        L.vr_last_error.argtypes = [C.c_void_p]
-        L.vr_last_error.restype = C.c_char_p
-        L.vr_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.vr_trajectory.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         n = len(sequences)
         assert (trackers.n == n and estimators.n == n) if batch_mode else (len(trackers) == n and len(estimators) == n)
-        self._keep = []  # arrays the session borrows
-        arr = (_Seq * n)()
+        self._keep = [trackers, estimators]  # the handles and arrays the session borrows
+        arr = (ReplaySequence * n)()
         for k, sq in enumerate(sequences):
             img = sq["images"]
             if isinstance(img, np.ndarray):
@@ -50,52 +35,34 @@ class ReplaySession:
                 arr[k].images, arr[k].images_on_device = int(img), 1
             arr[k].row_stride, arr[k].frame_stride, arr[k].n_images = w, h * w, nimg
             for name in ("stamps", "imu_t", "acc", "gyr"):
-                a = np.ascontiguousarray(sq[name], np.float64)
+                a = f64(sq[name])
                 self._keep.append(a)
                 setattr(arr[k], name, a.ctypes.data)
             arr[k].n_imu = len(sq["imu_t"])
         self._arr, self.n = arr, n
-        self.h = C.c_void_p()
         if batch_mode:
-            if L.vr_open_batch(trackers.h, estimators.h, arr, C.byref(self.h)) != 0:
-                raise RuntimeError("vr_open_batch failed")
+            self._open("vr_open_batch", trackers.h, estimators.h, arr)
         else:
-            th = (C.c_void_p * n)(*[t.h for t in trackers])
-            eh = (C.c_void_p * n)(*[e.h for e in estimators])
-            if L.vr_open(n, th, eh, arr, C.byref(self.h)) != 0:
-                raise RuntimeError("vr_open failed")
+            self._open("vr_open", n, (C.c_void_p * n)(*[t.h for t in trackers]), (C.c_void_p * n)(*[e.h for e in estimators]), arr)
 
     def advance(self, n_pub: int) -> int:
-        r = self.lib.vr_advance(self.h, n_pub)
-        if r < 0:
-            raise RuntimeError(f"vr_advance: {self.lib.vr_last_error(self.h).decode()} ({r})")
-        return r
+        return self._check(self.lib.vr_advance(self.h, n_pub))
 
     def queue_relo(self, seq: int, arrival_stamp, frame_stamp, frame_index, match_points, relo_t, relo_r):
         """A /pose_graph/match_points message for sequence seq (vr_queue_relo): applied before the first image at or after
         arrival_stamp, like process() drains relo_buf (estimator_node.cpp:266-291).  Not concurrently with advance()."""
-        mp = np.ascontiguousarray(match_points, np.float64).reshape(-1, 3)
-        t3 = np.ascontiguousarray(relo_t, np.float64).reshape(3)
-        r9 = np.ascontiguousarray(relo_r, np.float64).reshape(9)
-        self.lib.vr_queue_relo.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-        rc = self.lib.vr_queue_relo(self.h, seq, float(arrival_stamp), float(frame_stamp), int(frame_index), len(mp),
-                                    mp.ctypes.data_as(C.c_void_p), t3.ctypes.data_as(C.c_void_p), r9.ctypes.data_as(C.c_void_p))
-        if rc != 0:
-            raise RuntimeError(f"vr_queue_relo: {rc}")
+        mp, t3, r9 = f64(match_points).reshape(-1, 3), f64(relo_t).reshape(3), f64(relo_r).reshape(9)
+        self._check(self.lib.vr_queue_relo(self.h, seq, float(arrival_stamp), float(frame_stamp), int(frame_index), len(mp), ptr(mp),
+                                           ptr(t3), ptr(r9)))
 
     def stats(self, seq: int):
         f, l, a, b = C.c_int(0), C.c_longlong(0), C.c_double(0), C.c_double(0)
-        self.lib.vr_stats(self.h, seq, C.byref(f), C.byref(l), C.byref(a), C.byref(b))
+        self._check(self.lib.vr_stats(self.h, seq, C.byref(f), C.byref(l), C.byref(a), C.byref(b)))
         return dict(frames=f.value, launches=l.value, h2d=a.value, d2h=b.value)
 
     def trajectory(self, seq: int):
-        n = self.lib.vr_trajectory(self.h, seq, 0, None, None)
+        n = self._check(self.lib.vr_trajectory(self.h, seq, 0, None, None))
         t, p = np.zeros(n), np.zeros((n, 3))
         if n:
-            self.lib.vr_trajectory(self.h, seq, n, t.ctypes.data, p.ctypes.data)
+            self._check(self.lib.vr_trajectory(self.h, seq, n, ptr(t), ptr(p)))
         return t, p
-
-    def close(self):
-        if self.h:
-            self.lib.vr_close(self.h)
-            self.h = None

@@ -3,63 +3,10 @@ FeatureTracker (feature_tracker/src/feature_tracker.h:28-64)."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libvinsb200.so")
-_lib = None
-
-u8p, i32p, f32p = (C.POINTER(t) for t in (C.c_uint8, C.c_int, C.c_float))
-
-
-class TrackerConfig(C.Structure):
-    _fields_ = [("rows", C.c_int), ("cols", C.c_int), ("max_cnt", C.c_int), ("min_dist", C.c_int), ("freq", C.c_int),
-                ("equalize", C.c_int), ("fisheye", C.c_int), ("focal_length", C.c_int), ("f_threshold", C.c_double),
-                ("camera_model", C.c_int), ("intrinsics", C.c_double * 8), ("fisheye_mask", C.c_void_p),
-                ("device", C.c_int), ("xi", C.c_double)]
-
-
-def load_library():
-    """Loads libvinsb200.so.  Raises if it has not been built (python -m vins_mono_b200.build)."""
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} is missing: run `python vins_mono_b200/build.py` (no CPU fallback exists)")
-        lib = C.CDLL(LIB_PATH)
-        lib.vt_last_error.restype = C.c_char_p
-        lib.vt_last_error.argtypes = [C.c_void_p]
-        lib.vt_create.argtypes = [C.POINTER(TrackerConfig), C.POINTER(C.c_void_p)]
-        lib.vt_destroy.argtypes = [C.c_void_p]
-        lib.vt_read_image.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_int]
-        lib.vt_read_image_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_int]
-        lib.vt_count.argtypes = [C.c_void_p]
-        lib.vt_get.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        lib.vt_node_image.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
-        lib.vt_node_image_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
-        lib.vt_node_pack.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 6
-        lib.vt_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int)]
-        lib.vt_set_profile.argtypes = [C.c_void_p, C.c_int]
-        lib.vt_kernel_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.vt_last_traffic.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-        lib.vt_debug_equalized.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        lib.vt_debug_gftt.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p,
-                                      C.POINTER(C.c_int), C.c_void_p]
-        lib.vt_debug_lk.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p,
-                                    C.c_void_p]
-        lib.vt_batch_create.argtypes = [C.POINTER(TrackerConfig), C.c_int, C.POINTER(C.c_void_p)]
-        lib.vt_batch_destroy.argtypes = [C.c_void_p]
-        lib.vt_batch_member.argtypes = [C.c_void_p, C.c_int]
-        lib.vt_batch_member.restype = C.c_void_p
-        lib.vt_batch_last_error.argtypes = [C.c_void_p]
-        lib.vt_batch_last_error.restype = C.c_char_p
-        lib.vt_batch_read_image.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int]
-        lib.vt_batch_node_image.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-        lib.vt_batch_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int)]
-        lib.vt_batch_set_profile.argtypes = [C.c_void_p, C.c_int]
-        lib.vt_batch_kernel_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib = lib
-    return _lib
+from ._abi import LIB_PATH, Batch, Handle, TrackerConfig, load_library, ptr  # noqa: F401
 
 
 def _make_tracker_config(rows=480, cols=752, max_cnt=150, min_dist=30, freq=10, equalize=1, focal_length=460,
@@ -76,51 +23,29 @@ def _make_tracker_config(rows=480, cols=752, max_cnt=150, min_dist=30, freq=10, 
     return cfg, mask
 
 
-def _ptr(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
-
-
-class FeatureTracker:
+class FeatureTracker(Handle):
     """Drop-in for the reference FeatureTracker: readImage(img, t) then read the public result arrays."""
+    _destroy, _last_error = "vt_destroy", "vt_last_error"
 
     def __init__(self, **kw):
-        self.lib = load_library()
         cfg, self._mask = _make_tracker_config(**kw)
         self.cfg, self.rows, self.cols, self.max_cnt = cfg, cfg.rows, cfg.cols, cfg.max_cnt
-        h = C.c_void_p()
-        rc = self.lib.vt_create(C.byref(cfg), C.byref(h))
-        if rc != 0:
-            raise RuntimeError(f"vt_create failed with status {rc} (-2 = no CUDA device; this library has no CPU path)")
-        self.h = h
-        self._borrowed = False
         self.PUB_THIS_FRAME = False
+        self._open("vt_create", C.byref(cfg))
 
     @classmethod
-    def _member(cls, lib, handle, cfg):
-        self = cls.__new__(cls)
-        self.lib, self.cfg, self.rows, self.cols, self.max_cnt = lib, cfg, cfg.rows, cfg.cols, cfg.max_cnt
-        self.h, self._borrowed, self.PUB_THIS_FRAME, self._mask = C.c_void_p(handle), True, False, None
+    def _member(cls, batch, k):
+        self = cls._borrow(batch, batch.lib.vt_batch_member(batch.h, k))
+        self.cfg, self.rows, self.cols, self.max_cnt = batch.cfg, batch.cfg.rows, batch.cfg.cols, batch.cfg.max_cnt
+        self.PUB_THIS_FRAME, self._mask = False, None
         return self
-
-    def close(self):
-        if getattr(self, "h", None):
-            if not self._borrowed:
-                self.lib.vt_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _check(self, rc):
-        if rc < 0:
-            raise RuntimeError(f"vinsb200 error {rc}: {self.lib.vt_last_error(self.h).decode()}")
-        return rc
 
     # FeatureTracker::readImage(const cv::Mat&, double) + updateID loop; PUB_THIS_FRAME is the reference's global
     def readImage(self, img, cur_time, pub_this_frame=None):
         img = np.ascontiguousarray(img, np.uint8)
         assert img.shape == (self.rows, self.cols)
         pub = self.PUB_THIS_FRAME if pub_this_frame is None else pub_this_frame
-        self._check(self.lib.vt_read_image(self.h, _ptr(img), img.strides[0], float(cur_time), int(bool(pub))))
+        self._check(self.lib.vt_read_image(self.h, ptr(img), img.strides[0], float(cur_time), int(bool(pub))))
         return self.result()
 
     def read_image_device(self, dptr, stride, cur_time, pub):
@@ -130,7 +55,7 @@ class FeatureTracker:
         """img_callback: returns (ret, restart) with ret 0/1/2 as in vt_node_image."""
         img = np.ascontiguousarray(img, np.uint8)
         restart = C.c_int(0)
-        r = self._check(self.lib.vt_node_image(self.h, _ptr(img), img.strides[0], float(stamp), C.byref(restart)))
+        r = self._check(self.lib.vt_node_image(self.h, ptr(img), img.strides[0], float(stamp), C.byref(restart)))
         return r, restart.value
 
     def node_image_device(self, dptr, stride, stamp):
@@ -138,10 +63,10 @@ class FeatureTracker:
         return self._check(self.lib.vt_node_image_device(self.h, C.c_void_p(dptr), stride, float(stamp), C.byref(restart)))
 
     def result(self):
-        n = self.lib.vt_count(self.h)
+        n = self._check(self.lib.vt_count(self.h))
         ids, tc = np.zeros(n, np.int32), np.zeros(n, np.int32)
         cur, un, vel = (np.zeros((n, 2), np.float32) for _ in range(3))
-        self.lib.vt_get(self.h, _ptr(ids), _ptr(tc), _ptr(cur), _ptr(un), _ptr(vel))
+        self._check(self.lib.vt_get(self.h, ptr(ids), ptr(tc), ptr(cur), ptr(un), ptr(vel)))
         self.ids, self.track_cnt, self.cur_pts, self.cur_un_pts, self.pts_velocity = ids, tc, cur, un, vel
         return dict(ids=ids, track_cnt=tc, cur_pts=cur, un_pts=un, velocity=vel)
 
@@ -150,35 +75,35 @@ class FeatureTracker:
         cap = self.max_cnt
         xy = np.zeros((cap, 2), np.float32)
         ch = [np.zeros(cap, np.float32) for _ in range(5)]
-        n = self._check(self.lib.vt_node_pack(self.h, cap, _ptr(xy), *[_ptr(c) for c in ch]))
+        n = self._check(self.lib.vt_node_pack(self.h, cap, ptr(xy), *[ptr(c) for c in ch]))
         return {int(ch[0][i]): (float(xy[i, 0]), float(xy[i, 1]), 1.0, float(ch[1][i]), float(ch[2][i]),
                                 float(ch[3][i]), float(ch[4][i])) for i in range(n)}
 
     KERNEL_GROUPS = ["clahe", "pyrdown", "lk_track", "mask_discs", "min_eig", "gftt_tail"]
 
     def set_profile(self, on):
-        self.lib.vt_set_profile(self.h, int(on))
+        self._check(self.lib.vt_set_profile(self.h, int(on)))
 
     def kernel_times(self):
         ms, cnt = np.zeros(6), np.zeros(6, np.int32)
-        self.lib.vt_kernel_times(self.h, _ptr(ms), _ptr(cnt))
+        self._check(self.lib.vt_kernel_times(self.h, ptr(ms), ptr(cnt)))
         return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNEL_GROUPS)}
 
     def traffic(self):
         a, b = C.c_double(0), C.c_double(0)
-        self.lib.vt_last_traffic(self.h, C.byref(a), C.byref(b))
+        self._check(self.lib.vt_last_traffic(self.h, C.byref(a), C.byref(b)))
         return a.value, b.value
 
     def timing(self):
         ms, k = C.c_float(0), C.c_int(0)
-        self.lib.vt_last_timing(self.h, C.byref(ms), C.byref(k))
+        self._check(self.lib.vt_last_timing(self.h, C.byref(ms), C.byref(k)))
         return ms.value, k.value
 
     # --- single-stage access for parity tests ---
     def debug_level(self, level):
         out = np.zeros((self.rows, self.cols), np.uint8)
         r, c = C.c_int(0), C.c_int(0)
-        self._check(self.lib.vt_debug_equalized(self.h, level, _ptr(out), C.byref(r), C.byref(c)))
+        self._check(self.lib.vt_debug_equalized(self.h, level, ptr(out), C.byref(r), C.byref(c)))
         return out.ravel()[: r.value * c.value].reshape(r.value, c.value).copy()
 
     def debug_gftt(self, img, mask, max_corners, want_eig=False):
@@ -187,8 +112,8 @@ class FeatureTracker:
         out = np.zeros((max_corners, 2), np.float32)
         nc = C.c_int(0)
         eig = np.zeros((self.rows, self.cols), np.float32) if want_eig else None
-        n = self._check(self.lib.vt_debug_gftt(self.h, _ptr(img), img.strides[0], _ptr(mask), max_corners, _ptr(out),
-                                               C.byref(nc), _ptr(eig)))
+        n = self._check(self.lib.vt_debug_gftt(self.h, ptr(img), img.strides[0], ptr(mask), max_corners, ptr(out),
+                                               C.byref(nc), ptr(eig)))
         return out[:n].copy(), nc.value, eig
 
     def debug_lk(self, prev, nxt, pts):
@@ -196,33 +121,20 @@ class FeatureTracker:
         pts = np.ascontiguousarray(pts, np.float32)
         n = len(pts)
         out, st = np.zeros((n, 2), np.float32), np.zeros(n, np.uint8)
-        self._check(self.lib.vt_debug_lk(self.h, _ptr(prev), _ptr(nxt), prev.strides[0], _ptr(pts), n, _ptr(out), _ptr(st)))
+        self._check(self.lib.vt_debug_lk(self.h, ptr(prev), ptr(nxt), prev.strides[0], ptr(pts), n, ptr(out), ptr(st)))
         return out, st
 
 
-class TrackerBatch:
+class TrackerBatch(Batch):
     """n trackers advancing image by image together (include/vinsb200/tracker.h, vt_batch_*): one launch per kernel stage
     for the whole batch.  members[k] is a FeatureTracker mirror for result() / feature_message()."""
+    _destroy, _last_error = "vt_batch_destroy", "vt_batch_last_error"
 
     def __init__(self, n, **kw):
-        self.lib = load_library()
         self.cfg, self._mask = _make_tracker_config(**kw)
         self.n, self.rows, self.cols = n, self.cfg.rows, self.cfg.cols
-        h = C.c_void_p()
-        rc = self.lib.vt_batch_create(C.byref(self.cfg), n, C.byref(h))
-        if rc != 0:
-            raise RuntimeError(f"vt_batch_create failed with status {rc} (-2 = no CUDA device; this library has no CPU path)")
-        self.h = h
-        self.members = [FeatureTracker._member(self.lib, self.lib.vt_batch_member(h, k), self.cfg) for k in range(n)]
-
-    def close(self):
-        if getattr(self, "h", None):
-            for m in self.members:
-                m.h = None
-            self.lib.vt_batch_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        self._open("vt_batch_create", C.byref(self.cfg), n)
+        self.members = [FeatureTracker._member(self, k) for k in range(n)]
 
     def _pointers(self, imgs):
         n = self.n
@@ -241,34 +153,30 @@ class TrackerBatch:
                 ptrs[k], dev = int(im), 1
         return active, ptrs, keep, stride, dev
 
-    def _check(self, rc):
-        if rc < 0:
-            raise RuntimeError(f"vinsb200 batch error {rc}: {self.lib.vt_batch_last_error(self.h).decode()}")
-
     def readImage(self, imgs, cur_times, pubs):
         """imgs[k]: numpy frame, device pointer or None (member idles)."""
         active, ptrs, keep, stride, dev = self._pointers(imgs)
         t = np.ascontiguousarray(cur_times, np.float64)
         p = np.ascontiguousarray(pubs, np.int32)
-        self._check(self.lib.vt_batch_read_image(self.h, _ptr(active), ptrs, stride, _ptr(t), _ptr(p), dev))
+        self._check(self.lib.vt_batch_read_image(self.h, ptr(active), ptrs, stride, ptr(t), ptr(p), dev))
 
     def node_image(self, imgs, stamps):
         """img_callback for every member with a frame; returns (results, restarts) arrays (0 / 1 / 2 per member)."""
         active, ptrs, keep, stride, dev = self._pointers(imgs)
         t = np.ascontiguousarray(stamps, np.float64)
         res, rst = np.zeros(self.n, np.int32), np.zeros(self.n, np.int32)
-        self._check(self.lib.vt_batch_node_image(self.h, _ptr(active), ptrs, stride, _ptr(t), dev, _ptr(res), _ptr(rst)))
+        self._check(self.lib.vt_batch_node_image(self.h, ptr(active), ptrs, stride, ptr(t), dev, ptr(res), ptr(rst)))
         return res, rst
 
     def timing(self):
         ms, k = C.c_float(0), C.c_int(0)
-        self.lib.vt_batch_last_timing(self.h, C.byref(ms), C.byref(k))
+        self._check(self.lib.vt_batch_last_timing(self.h, C.byref(ms), C.byref(k)))
         return ms.value, k.value
 
     def set_profile(self, on):
-        self.lib.vt_batch_set_profile(self.h, int(on))
+        self._check(self.lib.vt_batch_set_profile(self.h, int(on)))
 
     def kernel_times(self):
         ms, cnt = np.zeros(6), np.zeros(6, np.int32)
-        self.lib.vt_batch_kernel_times(self.h, _ptr(ms), _ptr(cnt))
+        self._check(self.lib.vt_batch_kernel_times(self.h, ptr(ms), ptr(cnt)))
         return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(FeatureTracker.KERNEL_GROUPS)}
