@@ -26,6 +26,9 @@
  *   vp_loop_last_timing      device ms (CUDA events) of the last attach (blur, FAST, BRIEF) and of the last verification
  *                            launch chain (matching, hypotheses, refit).
  *
+ * A key frame loaded by vp_load (pose_graph.h) has a slot with its saved corners and descriptors and no window points:
+ * it can be `old` of vp_find_connection; as `cur` it matches nothing.
+ *
  * Errors return < 0 and change neither the graph nor any slot.  The vp_debug_* entries run one stage each on device 0
  * with no handle.
  */

@@ -76,6 +76,31 @@ int vp_info(vp_graph* g, int* out8, double* costs2);
 /* device milliseconds (CUDA events) of the last collected optimisation; launches = kernels it launched */
 int vp_last_timing(vp_graph* g, float* ms, int* launches);
 
+/* ---- Map save / load: savePoseGraph / loadPoseGraph (pose_graph.cpp:697-870) in the reference's files, byte for byte.
+ * prefix is POSE_GRAPH_SAVE_PATH: the files are prefix + "pose_graph.txt", prefix + <index> + "_keypoints.txt" and
+ * prefix + <index> + "_briefdes.dat" (plain concatenation).
+ *   vp_save  collects an optimisation in flight, then writes every key frame in index order (loaded ones included)
+ *            and returns the count.  The keypoints and descriptors are the slot's FAST corners, their normalised
+ *            coordinates and descriptors (loop_verify.h); a key frame without an attached slot, or a graph without loop
+ *            verification, gets a count of 0 and two empty files.  The graph does not change.
+ *   vp_load  on a graph with no key frame (as the node does at start-up, load_previous_pose_graph): every saved key
+ *            frame becomes key frame <row> of sequence 0 (rows numbered 0, 1, 2, ...) with its VIO and PG pose both
+ *            the saved PG pose (the rotation from the parsed quaternion, not normalised), its loop as stored (the gate
+ *            is not re-applied; the loops count in vp_info) and earliest_loop_index their smallest target.  Nothing is
+ *            optimised.  With loop verification enabled, each loaded key frame's slot receives its corners, normalised
+ *            corners (as parsed) and descriptors with no window points: it can be the old key frame of
+ *            vp_find_connection, and as the current one it matches nothing.  Without it only pose_graph.txt is read.
+ *            Returns the count.  The next vp_add_keyframe starts sequence 1, which is shifted onto the map at its first
+ *            accepted loop onto it.
+ * Key frames of sequence 0 are constant in every optimisation, and so are the loops between two of them; a loop onto
+ * one is not a free anchor and counts against no capacity.  vp_load errors (the graph and every slot stay as they were,
+ * vp_last_error names the file and line): a graph with key frames, a missing or unreadable file, a truncated or
+ * unparsable line, a row out of order, a loop_index not naming an earlier row, a descriptor line that is not 256 '0' /
+ * '1' characters and a keypoint count that does not match the files are VP_ERR_INVALID; more rows than max_keyframes
+ * or more keypoints than max_corners VP_ERR_CAPACITY.  A file vp_save cannot write is VP_ERR_INVALID. */
+int vp_save(vp_graph* g, const char* prefix);
+int vp_load(vp_graph* g, const char* prefix);
+
 /* ---- Batch: n independent graphs whose pending optimisations run in ONE launch chain (the member index is a grid
  * dimension), one host-to-device and one device-to-host copy for all of them.  A stand-alone handle from vp_create is a
  * batch of one running the same code.

@@ -145,6 +145,8 @@ SIGNATURES = {
     "vp_get_path": (I, [V, I] + [V] * 4),
     "vp_info": (I, [V, V, V]),
     "vp_last_timing": (I, [V, FP, IP]),
+    "vp_save": (I, [V, S]),
+    "vp_load": (I, [V, S]),
     "vp_batch_create": (I, [C.POINTER(PoseGraphConfig), I, VP]),
     "vp_batch_destroy": (None, [V]),
     "vp_batch_size": (I, [V]),

@@ -19,6 +19,7 @@
 #include "lv_kernels.h"
 #include "lv_layout.h"
 #include "pg_host.h"
+#include "pg_map.h"
 
 namespace vb {
 
@@ -54,6 +55,69 @@ struct LvState {
 };
 
 void lv_release(LvState* s) { delete s; }
+
+int lv_max_corners(const LvState* s) { return s->cfg.max_corners; }
+
+int lv_read_points(LvState* s, int member, std::vector<MapKeyFrame>* kfs, std::string* err) {
+    const int n = (int)kfs->size();
+    if (!n) return 0;
+    const LvSlotLayout sl = lv_slot_layout(s->cfg.max_window, s->cfg.max_corners);
+    const char* base = s->d_arena + (size_t)member * s->cap_kf * s->slot_bytes;
+    std::vector<LvSlotHdr> hdr(n);
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy2D(hdr.data(), sizeof(LvSlotHdr), base, s->slot_bytes, sizeof(LvSlotHdr), n, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n; i++) {
+        MapKeyFrame& k = (*kfs)[i];
+        const size_t c = s->attached[(size_t)member * s->cap_kf + i] ? (size_t)hdr[i].n_corners : 0;
+        k.n_kp = (int)c;
+        k.kp.resize(2 * c);
+        k.kpn.resize(2 * c);
+        k.desc.resize(4 * c);
+        if (!c) continue;
+        const char* slot = base + (size_t)i * s->slot_bytes;
+        VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy(k.kp.data(), slot + sl.kp, 8 * c, cudaMemcpyDeviceToHost));
+        VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy(k.kpn.data(), slot + sl.kpn, 8 * c, cudaMemcpyDeviceToHost));
+        VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy(k.desc.data(), slot + sl.kdesc, 32 * c, cudaMemcpyDeviceToHost));
+    }
+    return 0;
+}
+
+int lv_write_points(LvState* s, int member, int first, const std::vector<MapKeyFrame>& kfs, const double* P, const double* Q,
+                    std::string* err) {
+    const int n = (int)kfs.size();
+    if (!n) return 0;
+    size_t bytes = lv_load_jobs_bytes(n);
+    for (const MapKeyFrame& k : kfs) bytes += lv_load_layout(k.n_kp).total;
+    std::vector<char> h(bytes, 0);
+    long long* jobs = reinterpret_cast<long long*>(h.data());
+    size_t off = lv_load_jobs_bytes(n);
+    for (int i = 0; i < n; i++) {
+        const MapKeyFrame& k = kfs[i];
+        const LvLoadLayout ll = lv_load_layout(k.n_kp);
+        jobs[2 * i] = (long long)(((size_t)member * s->cap_kf + first + i) * s->slot_bytes);
+        jobs[2 * i + 1] = (long long)off;
+        LvSlotHdr hd{};
+        std::memcpy(hd.vio_P, P + 3 * i, sizeof(hd.vio_P));
+        std::memcpy(hd.vio_Q, Q + 4 * i, sizeof(hd.vio_Q));
+        hd.n_win = 0;
+        hd.n_corners = k.n_kp;
+        hd.attached = 1;
+        std::memcpy(h.data() + off, &hd, sizeof(hd));
+        std::memcpy(h.data() + off + ll.kp, k.kp.data(), 8 * (size_t)k.n_kp);
+        std::memcpy(h.data() + off + ll.kpn, k.kpn.data(), 8 * (size_t)k.n_kp);
+        std::memcpy(h.data() + off + ll.kdesc, k.desc.data(), 32 * (size_t)k.n_kp);
+        off += ll.total;
+    }
+    DeviceArray<char> d;
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, d.alloc(bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, s->stream));
+    launch_lv_scatter(s->d_arena, d, n, s->cfg.max_window, s->cfg.max_corners, s->stream);
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaGetLastError());
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaStreamSynchronize(s->stream));
+    for (int i = 0; i < n; i++) s->attached[(size_t)member * s->cap_kf + first + i] = 1;
+    return 0;
+}
 
 }  // namespace vb
 

@@ -674,7 +674,31 @@ __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char*
     }
 }
 
+// ---- vp_load: one CTA per loaded key frame copies its staged block into its slot (16-byte words; every array of both
+//      layouts is 16-byte aligned and the copies are whole words of the block, which the staging zero-pads)
+__global__ void __launch_bounds__(256) lv_scatter_kernel(char* arena, const char* staged, int max_window, int max_corners) {
+    const long long* job = reinterpret_cast<const long long*>(staged) + 2 * blockIdx.x;
+    char* slot = arena + job[0];
+    const char* blk = staged + job[1];
+    const LvSlotHdr h = *reinterpret_cast<const LvSlotHdr*>(blk);
+    const LvSlotLayout sl = lv_slot_layout(max_window, max_corners);
+    const LvLoadLayout ll = lv_load_layout(h.n_corners);
+    auto copy = [&](size_t dst, size_t src, size_t bytes) {
+        const uint4* s = reinterpret_cast<const uint4*>(blk + src);
+        uint4* d = reinterpret_cast<uint4*>(slot + dst);
+        for (size_t i = threadIdx.x; i < bytes / 16; i += blockDim.x) d[i] = s[i];
+    };
+    copy(0, 0, lv_align16(sizeof(LvSlotHdr)));
+    copy(sl.kp, ll.kp, lv_align16(8 * (size_t)h.n_corners));
+    copy(sl.kpn, ll.kpn, lv_align16(8 * (size_t)h.n_corners));
+    copy(sl.kdesc, ll.kdesc, 32 * (size_t)h.n_corners);
+}
+
 }  // namespace
+
+void launch_lv_scatter(char* arena, const char* staged, int n_kf, int max_window, int max_corners, cudaStream_t s) {
+    if (n_kf > 0) lv_scatter_kernel<<<n_kf, 256, 0, s>>>(arena, staged, max_window, max_corners);
+}
 
 void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s) {
     Intr in;

@@ -25,6 +25,10 @@ int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev);
 // The corner lift alone: the status and the corners kp already in scratch and slot.
 void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s);
 
+// Loaded key frames into their slots (vp_load): staged (device) holds n_kf jobs and blocks as lv_load_layout defines them;
+// each block's header, corners, normalised corners and descriptors go to its slot.  One launch.
+void launch_lv_scatter(char* arena, const char* staged, int n_kf, int max_window, int max_corners, cudaStream_t s);
+
 // n_jobs verifications.  jobs (device): per job the slot byte offsets of cur and old in the arena (2 x long long).
 // Scratch (lv_conn_layout) and result (lv_result_doubles) per job at the given strides.
 struct LvConnLaunch {

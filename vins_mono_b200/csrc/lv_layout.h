@@ -76,6 +76,23 @@ LV_LAYOUT_FN LvStageLayout lv_stage_layout(int rows, int cols, int max_window) {
     return o;
 }
 
+// ---- staging of the key frames one vp_load puts into their slots (one host-to-device copy), in bytes: per key frame a
+//      job (slot byte offset in the arena, block byte offset in the staging buffer: 2 x long long) | per key frame a
+//      block of n corners: header (n_win 0) | corners (float x 2) | corners normalised (float x 2) | descriptors
+struct LvLoadLayout {
+    size_t hdr, kp, kpn, kdesc, total;
+};
+LV_LAYOUT_FN size_t lv_load_jobs_bytes(int n_kf) { return lv_align16(16 * (size_t)n_kf); }
+LV_LAYOUT_FN LvLoadLayout lv_load_layout(int n) {
+    const size_t c = (size_t)n;
+    LvLoadLayout o{0, 0, 0, 0, 0};
+    o.kp = lv_align16(sizeof(LvSlotHdr));
+    o.kpn = o.kp + lv_align16(8 * c);
+    o.kdesc = o.kpn + lv_align16(8 * c);
+    o.total = o.kdesc + lv_align16(32 * c);
+    return o;
+}
+
 // ---- scratch of one attach, in bytes: blurred image | FAST score map | survivor map | survivors per row |
 //      status (corner count, overflow)
 struct LvAttachLayout {

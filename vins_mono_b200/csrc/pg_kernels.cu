@@ -4,10 +4,13 @@
 // tolerances 1e-6 / 1e-8 / 1e-10).  float64 throughout, no atomics: every sum has a fixed order, so runs are
 // bit-reproducible and a batch member computes exactly what a stand-alone handle computes.
 //
-// Parameters: per key frame of the range yaw (degrees, NormalizeAngle on update) and t; local key frame 0 (the earliest
-// loop anchor) is constant.  The damped normal equations are solved exactly with this structure:
-//   chain   the free key frames in super-blocks of 4 by local index (16 unknowns each).  Sequential edges reach back at
-//           most 4 key frames, so their part of the system is block-tridiagonal.
+// Parameters: per key frame of the range yaw (degrees, NormalizeAngle on update) and t; local key frames 0 .. nc - 1 are
+// constant (the earliest loop anchor, or the key frames of a loaded map that share an edge with a free one; the host
+// packs no edge between two constants, see pose_graph.cpp).  The damped normal equations are solved exactly with this
+// structure:
+//   chain   the free key frames in super-blocks of 4 by local index (16 unknowns each), from the super-block holding
+//           local nc on: the super-blocks before it hold constants only.  Sequential edges reach back at most 4 key
+//           frames, so their part of the system is block-tridiagonal.
 //   border  the free loop anchors (old ends of loop edges), 4 columns each, D of them.  Their rows and columns are
 //           identity rows in the chain; every loop edge has an end in the border or a constant end.
 //   step 1  block Cholesky along the chain (pg_chain_kernel, ceil((D + 1) / 384) CTAs per member), carrying
@@ -90,7 +93,7 @@ __device__ double four_dof_eval(const double* xi, const double* xj, double pitch
 }
 
 struct PgView {
-    int n, nb, D, Dp, nsb;
+    int n, nb, nc, D, Dp, nsb;
     const double *pose, *loopm;
     const int *seq, *loop, *bslot, *lfirst, *lnext, *anchors;
     PgState* st;
@@ -106,6 +109,7 @@ __device__ PgView pg_view(const PgLaunch& a, int slot) {
     PgView v;
     v.n = reinterpret_cast<const int*>(a.d_in + h.n)[slot];
     v.nb = reinterpret_cast<const int*>(a.d_in + h.nb)[slot];
+    v.nc = reinterpret_cast<const int*>(a.d_in + h.nc)[slot];
     v.D = 4 * v.nb;
     v.Dp = v.D + 1;
     v.nsb = pg_num_sb(v.n);
@@ -131,10 +135,10 @@ __device__ PgView pg_view(const PgLaunch& a, int slot) {
     return v;
 }
 
-// kind of a local key frame: 0 chain (free, not an anchor), 1 border (free anchor), 2 constant (local 0), 3 padding
+// kind of a local key frame: 0 chain (free, not an anchor), 1 border (free anchor), 2 constant (local < nc), 3 padding
 __device__ __forceinline__ int kf_kind(const PgView& v, int k) {
     if (k >= v.n) return 3;
-    if (k == 0) return 2;
+    if (k < v.nc) return 2;
     return v.bslot[k] >= 0 ? 1 : 0;
 }
 
@@ -274,7 +278,7 @@ __global__ void __launch_bounds__(256) pg_linearize_kernel(PgLaunch a) {
         }
         for (int p = 0; p < 4; p++) {
             v.g[4 * k + p] = g[p];
-            if (k > 0) gmax = fmax(gmax, fabs(g[p]));
+            if (k >= v.nc) gmax = fmax(gmax, fabs(g[p]));
             if (v.st->first) v.scale[4 * k + p] = 1.0 / (1.0 + sqrt(H[5 * p]));
         }
     }
@@ -323,6 +327,8 @@ __device__ __forceinline__ double damped(double h, double radius) { return h + f
 // ---- step 1: block Cholesky along the chain; thread c < D + 1 carries border column c (c = D: the right-hand side).
 //      The columns spread over ceil((D + 1) / 384) CTAs (grid.x; grid.y is the member slot).  Every CTA repeats the
 //      super-block factorisation, which is deterministic, so all compute the same bits; CTA 0 alone stores L and F.
+//      The chain starts at super-block s0 = nc / 4: the earlier ones are identity blocks that couple to nothing (their
+//      F blocks into s0 are zero), so neither L, F nor W is formed for them.
 __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
     __shared__ double Lp[16][17], Lc[16][17], Fs[16][17], M[16][17];
     __shared__ int fail;
@@ -339,8 +345,9 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
     for (int k = 0; k < 16; k++) w[k] = 0.0;
     bool started = false;
     int start = v.nsb;
+    const int s0 = v.nc / PG_SB;
     if (tid == 0) fail = 0;
-    for (int s = 0; s < v.nsb; s++) {
+    for (int s = s0; s < v.nsb; s++) {
         for (int e = tid; e < 256; e += blockDim.x) {
             const int r = e >> 4, cc = e & 15, ka = 4 * s + (r >> 2), kb = 4 * s + (cc >> 2), kc = 4 * (s - 1) + (cc >> 2);
             double m = (r == cc) ? 1.0 : 0.0;
@@ -352,7 +359,7 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
             Fs[r][cc] = (s > 0 && kf_kind(v, ka) == 0 && kf_kind(v, kc) == 0 && ka - kc <= 4) ? h_entry(v, ka, kc, r & 3, cc & 3) : 0.0;
         }
         __syncthreads();
-        if (s > 0) {
+        if (s > s0) {
             if (tid < 16) {  // F = E L_{s-1}^-T, one row per thread
                 const int r = tid;
                 for (int q = 0; q < 16; q++) {
@@ -421,7 +428,7 @@ __global__ void __launch_bounds__(384) pg_chain_kernel(PgLaunch a) {
 #pragma unroll
                 for (int k = 0; k < 16; k++) {
                     double val = b[k];
-                    if (s > 0)
+                    if (s > s0)
 #pragma unroll
                         for (int t = 0; t < 16; t++) val -= Fs[k][t] * w[t];
                     b[k] = val;
@@ -510,7 +517,7 @@ __device__ __forceinline__ void chain_back_substitute(const PgView& v, const dou
     const int tid = threadIdx.x, D = v.D, Dp = v.Dp;
     if (tid < 16) xn[tid] = 0.0;
     const int wid = tid >> 5, lane = tid & 31;
-    for (int s = v.nsb - 1; s >= 0; s--) {
+    for (int s = v.nsb - 1; s >= v.nc / PG_SB; s--) {
         for (int e = tid; e < 256; e += blockDim.x) {
             Ls[e >> 4][e & 15] = v.L[256 * s + e];
             Fn[e >> 4][e & 15] = (s + 1 < v.nsb) ? v.F[256 * (s + 1) + e] : 0.0;
@@ -799,7 +806,7 @@ __global__ void __launch_bounds__(256) pg_update_kernel(PgLaunch a) {
     for (int k = threadIdx.x; k < v.n; k += blockDim.x) {
         const double* x = v.x + 4 * k;
         double* xc = v.xc + 4 * k;
-        if (k == 0) {
+        if (k < v.nc) {
             for (int p = 0; p < 4; p++) xc[p] = x[p];
             continue;
         }
@@ -821,7 +828,7 @@ __global__ void __launch_bounds__(256) pg_update_kernel(PgLaunch a) {
             edge_eval(v, v.x, k, e, b, r, J);
             const double* di = v.dx + 4 * b;
             const double* dj = v.dx + 4 * k;
-            const bool fi = b > 0;
+            const bool fi = b >= v.nc;
             for (int t = 0; t < 4; t++) {
                 double jd = 0;
                 for (int p = 0; p < 4; p++) jd += (fi ? J[8 * t + p] * di[p] : 0.0) + J[8 * t + 4 + p] * dj[p];

@@ -57,18 +57,20 @@ PG_LAYOUT_FN PgInLayout pg_in_layout(int n, int nb) {
 }
 
 // ---- the batch input arena of one launch, in bytes: header | member blocks.  The header lists, per active slot b
-//      (grid.y of every kernel), the member index, n, nb and the byte / double offsets of its input and output blocks.
+//      (grid.y of every kernel), the member index, n, nb, the byte / double offsets of its input and output blocks and
+//      nc, the number of constant key frames (local 0 .. nc - 1; every other key frame is free).
 struct PgHdrLayout {
-    size_t member, n, nb, in_off, out_off, total;
+    size_t member, n, nb, in_off, out_off, nc, total;
 };
 PG_LAYOUT_FN PgHdrLayout pg_hdr_layout(int S) {
-    PgHdrLayout o{0, 0, 0, 0, 0, 0};
+    PgHdrLayout o{0, 0, 0, 0, 0, 0, 0};
     o.member = pg_align16(sizeof(int));  // [0] = number of active slots
     o.n = o.member + pg_align16((size_t)S * sizeof(int));
     o.nb = o.n + pg_align16((size_t)S * sizeof(int));
     o.in_off = o.nb + pg_align16((size_t)S * sizeof(int));
     o.out_off = o.in_off + pg_align16((size_t)S * sizeof(long long));
-    o.total = o.out_off + pg_align16((size_t)S * sizeof(long long));
+    o.nc = o.out_off + pg_align16((size_t)S * sizeof(long long));
+    o.total = o.nc + pg_align16((size_t)S * sizeof(int));
     return o;
 }
 // bytes of the arena: the header plus every member at capacity

@@ -17,6 +17,7 @@
 #include "pg_host.h"
 #include "pg_kernels.h"
 #include "pg_layout.h"
+#include "pg_map.h"
 
 using hm::Mat3;
 using hm::Quat;
@@ -58,9 +59,12 @@ struct vp_graph {
     Vec3 w_t_vio, t_drift;
     double yaw_drift = 0;
     int earliest_loop_index = -1, pending = -1, n_loops = 0, n_opt = 0;
-    // the optimisation in flight (enqueued, not collected): its range, the pitch / roll it used, its output once copied
+    int n_map = 0;  // key frames 0 .. n_map - 1 came from vp_load: sequence 0, constant in every optimisation
+    // the optimisation in flight (enqueued, not collected): its range, the key frames it packed (global index by local
+    // index), the pitch / roll it used, its output once copied
     bool inflight = false, ready = false;
     int inf_first = 0, inf_cur = 0, inf_D = 0;
+    std::vector<int> inf_map;
     std::vector<double> inf_pr, inf_out;
     int last_info[4] = {0, 0, 0, 0};
     double last_cost[2] = {0, 0};
@@ -103,7 +107,7 @@ int batch_wait(vp_batch* b) {
     b->ms[1] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - b->t0).count();
     for (size_t s = 0; s < b->slots.size(); s++) {
         vp_graph* g = b->members[b->slots[s]];
-        const int n = g->inf_cur - g->inf_first + 1;
+        const int n = (int)g->inf_map.size();
         const double* o = b->h_out + b->slot_out[s];
         g->inf_out.assign(o, o + vb::pg_out_layout(n).total);
         g->ready = true;
@@ -124,16 +128,23 @@ int collect(vp_graph* g) {
             return rc;
         }
     }
-    const int first = g->inf_first, cur = g->inf_cur, n = cur - first + 1;
+    const int first = g->inf_first, cur = g->inf_cur, n = (int)g->inf_map.size();
     if (!g->ready || g->inf_out.size() != vb::pg_out_layout(n).total) {
         g->err = "vp: the optimisation in flight has no result";
         return VP_ERR_CUDA;
     }
     const double* o = g->inf_out.data();
     for (int i = 0; i < n; i++) {
-        KeyFrame& kf = g->kfs[first + i];
+        KeyFrame& kf = g->kfs[g->inf_map[i]];
+        if (kf.seq == 0) continue;
         kf.R = hm::ypr2R(Vec3(o[4 * i], g->inf_pr[2 * i], g->inf_pr[2 * i + 1]));
         kf.P = Vec3(o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
+    }
+    // the loaded map's key frames of the range, packed or not: updatePose(t, ypr2R(euler)) of a constant block
+    for (int k = first; k < g->n_map; k++) {
+        KeyFrame& kf = g->kfs[k];
+        kf.R = hm::ypr2R(hm::R2ypr(Quat::FromR(kf.vio_R).R()));
+        kf.P = kf.vio_P;
     }
     const KeyFrame& ck = g->kfs[cur];
     g->yaw_drift = hm::R2ypr(ck.R).x - hm::R2ypr(ck.vio_R).x;
@@ -145,7 +156,7 @@ int collect(vp_graph* g) {
         kf.R = g->r_drift * kf.vio_R;
     }
     const double* sm = o + vb::pg_out_layout(n).summary;
-    g->last_info[0] = n;
+    g->last_info[0] = cur - first + 1;
     g->last_info[1] = g->inf_D;
     g->last_info[2] = (int)sm[0];
     g->last_info[3] = (int)sm[1];
@@ -198,14 +209,42 @@ int batch_create(const vp_config* cfg, int n, vp_batch** out) {
 
 // Packs member g's pending optimisation into the input arena at byte offset `off`.  Fails (changing nothing) when its
 // range has more free loop anchors than the graph's anchor capacity.
-// pr (out) receives the pitch and roll of each key frame of the range (the constants of the solve).  The member itself is
-// not changed.
-int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, std::vector<double>* pr) {
-    const int first = g->earliest_loop_index, cur = g->pending, n = cur - first + 1;
+// The range [first, cur] is packed as the solve's local key frames 0 .. n - 1, the nc constant ones first:
+//   - without a loaded map in the range (first >= n_map), the range itself; local 0 (first) is the one constant.
+//   - with one (first < n_map), the map key frames first .. n_map - 1 are constant, and so are the edges between two of
+//     them (sequential edges inside the map, loops stored with it): Ceres drops those from the minimiser.  Only the map
+//     key frames that a free key frame's loop lands on are packed, in ascending order and each with a sequence of its
+//     own (-1 - j), so that no sequential edge pairs two of them; the free key frames n_map .. cur follow.  The chain's
+//     serial work then grows with the free key frames only.
+// map (out) receives the global index of each local key frame, pr the pitch and roll of each (the constants of the
+// solve).  The member itself is not changed.
+int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, int* nc_out, std::vector<int>* map, std::vector<double>* pr) {
+    const int first = g->earliest_loop_index, cur = g->pending;
+    std::vector<int>& gl = *map;
+    gl.clear();
+    int nc = 1, seq_base = first;  // local i >= nc holds global seq_base + i - nc
+    if (first < g->n_map) {
+        for (int k = g->n_map; k <= cur; k++) {
+            const KeyFrame& kf = g->kfs[k];
+            if (kf.has_loop && kf.loop_index < g->n_map) gl.push_back(kf.loop_index);
+        }
+        std::sort(gl.begin(), gl.end());
+        gl.erase(std::unique(gl.begin(), gl.end()), gl.end());
+        nc = (int)gl.size();
+        seq_base = g->n_map;
+    } else {
+        gl.push_back(first);
+        seq_base = first + 1;
+    }
+    for (int k = seq_base; k <= cur; k++) gl.push_back(k);
+    const int n = (int)gl.size();
+    auto local = [&](int k) {
+        return k >= seq_base ? nc + k - seq_base : (int)(std::lower_bound(gl.begin(), gl.begin() + nc, k) - gl.begin());
+    };
     std::vector<int> anchors;
-    for (int i = 0; i < n; i++) {
-        const KeyFrame& kf = g->kfs[first + i];
-        if (kf.has_loop && kf.loop_index - first > 0) anchors.push_back(kf.loop_index - first);
+    for (int i = nc; i < n; i++) {
+        const KeyFrame& kf = g->kfs[gl[i]];
+        if (kf.has_loop && local(kf.loop_index) >= nc) anchors.push_back(local(kf.loop_index));
     }
     std::sort(anchors.begin(), anchors.end());
     anchors.erase(std::unique(anchors.begin(), anchors.end()), anchors.end());
@@ -215,6 +254,7 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, st
         g->err = "vp_optimize: " + std::to_string(nb) + " free loop anchors in the optimised range, at most " + std::to_string(cap);
         return VP_ERR_CAPACITY;
     }
+    const bool map_range = first < g->n_map;
     const vb::PgInLayout il = vb::pg_in_layout(n, nb);
     char* in = base + off;
     double* pose = reinterpret_cast<double*>(in + il.pose);
@@ -228,15 +268,16 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, st
     std::vector<int> last(n, -1);
     pr->resize(2 * (size_t)n);
     for (int i = 0; i < n; i++) {
-        const KeyFrame& kf = g->kfs[first + i];
+        const KeyFrame& kf = g->kfs[gl[i]];
+        const bool packed_edges = !map_range || i >= nc;  // a packed map key frame owns no edge
         const Quat q = Quat::FromR(kf.vio_R);
         const double p[7] = {kf.vio_P.x, kf.vio_P.y, kf.vio_P.z, q.w, q.x, q.y, q.z};
         std::memcpy(pose + 7 * i, p, sizeof(p));
         const Vec3 ypr = hm::R2ypr(q.R());
         (*pr)[2 * i] = ypr.y;
         (*pr)[2 * i + 1] = ypr.z;
-        seq[i] = kf.seq;
-        loop[i] = kf.has_loop ? kf.loop_index - first : -1;
+        seq[i] = packed_edges ? kf.seq : -1 - i;
+        loop[i] = packed_edges && kf.has_loop ? local(kf.loop_index) : -1;
         loopm[4 * i] = kf.loop_info[0];
         loopm[4 * i + 1] = kf.loop_info[1];
         loopm[4 * i + 2] = kf.loop_info[2];
@@ -257,6 +298,7 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, st
     }
     *n_out = n;
     *nb_out = nb;
+    *nc_out = nc;
     return 0;
 }
 
@@ -288,10 +330,12 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
     int* h_nb = reinterpret_cast<int*>(b->h_in + hl.nb);
     long long* h_in_off = reinterpret_cast<long long*>(b->h_in + hl.in_off);
     long long* h_out_off = reinterpret_cast<long long*>(b->h_in + hl.out_off);
+    int* h_nc = reinterpret_cast<int*>(b->h_in + hl.nc);
     // the members of this launch; their state changes only once the whole chain has been enqueued
     struct Slot {
         int k, nb;
         long long out_off;
+        std::vector<int> map;
         std::vector<double> pr;
     };
     std::vector<Slot> slots;
@@ -300,9 +344,10 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
         vp_graph* g = b->members[k];
         if ((active && !active[k]) || g->pending < 0) continue;
         int rc = collect(g);  // the member's previous result first
-        int n = 0, nb = 0;
+        int n = 0, nb = 0, nc = 0;
+        std::vector<int> map;
         std::vector<double> pr;
-        if (!rc) rc = pack_member(g, b->h_in, off, &n, &nb, &pr);
+        if (!rc) rc = pack_member(g, b->h_in, off, &n, &nb, &nc, &map, &pr);
         if (rc) {
             if (status) status[k] = rc;
             if (!first_err) first_err = rc;
@@ -311,9 +356,10 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
         h_member[count] = k;
         h_n[count] = n;
         h_nb[count] = nb;
+        h_nc[count] = nc;
         h_in_off[count] = (long long)off;
         h_out_off[count] = (long long)out_off;
-        slots.push_back(Slot{k, nb, (long long)out_off, std::move(pr)});
+        slots.push_back(Slot{k, nb, (long long)out_off, std::move(map), std::move(pr)});
         off += vb::pg_in_layout(n, nb).total;
         out_off += vb::pg_out_layout(n).total;
         max_n = std::max(max_n, n);
@@ -344,6 +390,7 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
         g->inf_first = g->earliest_loop_index;
         g->inf_cur = g->pending;
         g->inf_D = 4 * sl.nb;
+        g->inf_map = std::move(sl.map);
         g->inf_pr = std::move(sl.pr);
         g->pending = -1;
         if (status) status[sl.k] = 1;
@@ -572,6 +619,77 @@ int vp_last_timing(vp_graph* g, float* ms, int* launches) {
     if (ms) *ms = g->last_ms;
     if (launches) *launches = g->last_launches;
     return 0;
+}
+
+int vp_save(vp_graph* g, const char* prefix) {
+    if (!g || !prefix) return VP_ERR_INVALID;
+    const int rc = collect(g);
+    if (rc) return rc;
+    std::vector<vb::MapKeyFrame> mk(g->kfs.size());
+    for (size_t i = 0; i < mk.size(); i++) {
+        const KeyFrame& kf = g->kfs[i];
+        vb::MapKeyFrame& m = mk[i];
+        m.index = (int)i;
+        m.stamp = kf.stamp;
+        KeyFrame v;
+        v.P = kf.vio_P;
+        v.R = kf.vio_R;
+        store_pose(v, m.vio_T, m.vio_Q);
+        store_pose(kf, m.pg_T, m.pg_Q);
+        m.loop_index = kf.has_loop ? kf.loop_index : -1;
+        std::memcpy(m.loop_info, kf.loop_info, sizeof(m.loop_info));
+    }
+    vb::LvState* lv = *vb::pg_loop_state(g->owner);
+    if (lv) {
+        const int r = vb::lv_read_points(lv, g->member, &mk, &g->err);
+        if (r) return r;
+    }
+    const int w = vb::map_write(prefix, mk, lv != nullptr, &g->err);
+    return w ? w : (int)mk.size();
+}
+
+int vp_load(vp_graph* g, const char* prefix) {
+    if (!g || !prefix) return VP_ERR_INVALID;
+    if (!g->kfs.empty()) {
+        g->err = "vp_load: the graph already holds key frames; a map is loaded before the first key frame";
+        return VP_ERR_INVALID;
+    }
+    vb::LvState* lv = *vb::pg_loop_state(g->owner);
+    std::vector<vb::MapKeyFrame> mk;
+    int rc = vb::map_read(prefix, lv != nullptr, g->cfg.max_keyframes, lv ? vb::lv_max_corners(lv) : 0, &mk, &g->err);
+    if (rc) return rc;
+    // the loaded-key-frame constructor (keyframe.cpp:44-70): the VIO pose is the saved PG pose, the rotation is
+    // toRotationMatrix of the parsed quaternion as it is (not normalised)
+    const int n = (int)mk.size();
+    std::vector<KeyFrame> kfs(n);
+    std::vector<double> P(3 * (size_t)n), Q(4 * (size_t)n);
+    int earliest = -1, loops = 0;
+    for (int i = 0; i < n; i++) {
+        const vb::MapKeyFrame& m = mk[i];
+        KeyFrame& kf = kfs[i];
+        kf.stamp = m.stamp;
+        kf.seq = 0;
+        kf.P = kf.vio_P = Vec3(m.pg_T[0], m.pg_T[1], m.pg_T[2]);
+        kf.R = kf.vio_R = Quat(m.pg_Q[0], m.pg_Q[1], m.pg_Q[2], m.pg_Q[3]).R();
+        kf.has_loop = m.loop_index != -1;
+        kf.loop_index = m.loop_index;
+        std::memcpy(kf.loop_info, m.loop_info, sizeof(kf.loop_info));
+        if (kf.has_loop) {
+            loops++;
+            if (earliest == -1 || m.loop_index < earliest) earliest = m.loop_index;
+        }
+        std::memcpy(&P[3 * (size_t)i], m.pg_T, sizeof(m.pg_T));
+        std::memcpy(&Q[4 * (size_t)i], m.pg_Q, sizeof(m.pg_Q));
+    }
+    if (lv) {
+        rc = vb::lv_write_points(lv, g->member, 0, mk, P.data(), Q.data(), &g->err);
+        if (rc) return rc;
+    }
+    g->kfs = std::move(kfs);
+    g->n_map = n;
+    g->earliest_loop_index = earliest;
+    g->n_loops = loops;
+    return n;
 }
 
 int vp_batch_create(const vp_config* cfg, int n, vp_batch** out) {

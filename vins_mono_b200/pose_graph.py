@@ -72,6 +72,16 @@ class PoseGraph(Handle):
         d["initial_cost"], d["final_cost"] = float(c[0]), float(c[1])
         return d
 
+    def save(self, prefix):
+        """savePoseGraph into prefix + "pose_graph.txt", prefix + <i> + "_keypoints.txt", prefix + <i> + "_briefdes.dat".
+        Returns the number of key frames written."""
+        return self._check(self.lib.vp_save(self.h, str(prefix).encode()))
+
+    def load(self, prefix):
+        """loadPoseGraph into a graph with no key frame: the saved key frames become sequence 0, constant in every
+        optimisation.  Returns the number of key frames loaded."""
+        return self._check(self.lib.vp_load(self.h, str(prefix).encode()))
+
     def timing(self):
         ms, n = C.c_float(), C.c_int()
         self._check(self.lib.vp_last_timing(self.h, C.byref(ms), C.byref(n)))
