@@ -9,9 +9,12 @@
  *   estimator_node.cpp:167-172       feature_callback drops the very first feature message
  *   estimator_node.cpp:225-265       process(): per-sample dt, linear interpolation of the sample that straddles the stamp
  *   estimator_node.cpp:275-316       image map construction and Estimator::processImage
- * The reference runs the two loops in two processes; here every sequence gets one tracker thread and one estimator
- * thread coupled by a bounded queue (depth 2), and any number of sequences run concurrently on one GPU (each handle
- * owns its CUDA stream).  No ROS, no CPU fallback: the handles are the CUDA ones of tracker.h / estimator.h.
+ * The reference runs the two loops in two processes.  Here a session is a list of lanes.  A lane is a contiguous run of
+ * sequences with one tracker thread and one estimator thread, coupled by a bounded queue (depth 2); all lanes run
+ * concurrently on one GPU (each handle owns its CUDA stream).  vr_open makes a lane per sequence, vr_open_batch one lane
+ * of all its sequences.  Both run the same two loops, which differ only in the library call of a step: a lane of one
+ * calls its sequence's own handles, a batch lane steps all its sequences with one batch call.  No ROS, no CPU fallback:
+ * the handles are the CUDA ones of tracker.h / estimator.h.
  */
 #ifndef VINSB200_REPLAY_H
 #define VINSB200_REPLAY_H
@@ -44,9 +47,9 @@ typedef struct vr_session vr_session;
  * before the first vr_advance. */
 int vr_open(int n_seq, vt_tracker* const* trackers, ve_estimator* const* estimators, const vr_sequence* seqs, vr_session** out);
 /* Batch mode: the sequences are the members of one tracker batch and one estimator batch (same count, same order; all
- * sequences with the same row_stride and images_on_device).  The session then runs ONE tracker loop and ONE estimator loop:
- * every image step is a vt_batch_node_image call, every published step a ve_batch_process_image call (one launch chain for all
- * sequences); vr_stats reports the batch's kernel launches on sequence 0. */
+ * sequences with the same row_stride and images_on_device).  The session is then ONE lane: every image step is a
+ * vt_batch_node_image call, every published step a ve_batch_process_image call (one launch chain for all sequences);
+ * vr_stats reports the batch's kernel launches on sequence 0. */
 int vr_open_batch(vt_batch* trackers, ve_batch* estimators, const vr_sequence* seqs, vr_session** out);
 void vr_close(vr_session* s);
 const char* vr_last_error(const vr_session* s);

@@ -1,9 +1,11 @@
-// Offline replay driver: the tracker node loop and the estimator node loop of the reference around the CUDA handles,
-// one thread pair per sequence, any number of sequences concurrently.  See include/vinsb200/replay.h for the mapping
-// to feature_tracker_node.cpp / estimator_node.cpp.  Pure host code on top of the two C ABIs.
+// Offline replay driver: the tracker node loop and the estimator node loop of the reference around the CUDA handles.  A
+// session is a list of lanes, each driven by one tracker thread and one estimator thread, and all lanes run concurrently.
+// See include/vinsb200/replay.h for the mapping to feature_tracker_node.cpp / estimator_node.cpp.  Pure host code on top of
+// the two C ABIs.
 #include "vinsb200/replay.h"
 
 #include <cstdio>
+#include <cstring>
 
 #include "host_math.h"
 
@@ -21,26 +23,31 @@ struct FeatureMsg {
     double stamp = 0;
     std::vector<int> ids;
     std::vector<double> obs;  // n x 7: x y z u v vx vy
-    long long launches = 0;
-    double h2d = 0, d2h = 0;
-    bool end = false;  // producer is done for this vr_advance call
+    double h2d = 0, d2h = 0;  // tracker traffic of the sequence's images since its previous message
 };
 
-struct Channel {  // bounded queue between the two loops of one sequence
+struct Step {  // what one image step of a lane's tracker loop produced: at most one feature message per sequence
+    std::vector<FeatureMsg> msgs;
+    std::vector<char> has;
+    long long launches = 0;  // tracker launches of the lane since its previous step
+    bool end = false;        // producer is done for this vr_advance call
+};
+
+struct Channel {  // bounded queue between the two loops of one lane
     std::mutex m;
     std::condition_variable cv;
-    std::deque<FeatureMsg> q;
+    std::deque<Step> q;
     size_t depth = 2;
-    void put(FeatureMsg&& v) {
+    void put(Step&& v) {
         std::unique_lock<std::mutex> lk(m);
         cv.wait(lk, [&] { return q.size() < depth; });
         q.push_back(std::move(v));
         cv.notify_all();
     }
-    FeatureMsg get() {
+    Step get() {
         std::unique_lock<std::mutex> lk(m);
         cv.wait(lk, [&] { return !q.empty(); });
-        FeatureMsg v = std::move(q.front());
+        Step v = std::move(q.front());
         q.pop_front();
         cv.notify_all();
         return v;
@@ -57,7 +64,7 @@ struct SeqState {
     double current_time = -1; // estimator_node.cpp:221
     double last_acc[3] = {0, 0, 0}, last_gyr[3] = {0, 0, 0};
     int frames = 0;
-    long long launches = 0;
+    long long launches = 0;   // a lane's kernel launches count on its first sequence: a batch's are not attributable to a member
     double h2d = 0, d2h = 0;
     std::vector<double> traj_t, traj_p;
     struct ReloMsg {  // a /pose_graph/match_points message waiting in relo_buf (estimator_node.cpp:22, 200-206)
@@ -67,47 +74,26 @@ struct SeqState {
         double relo_t[3], relo_r[9];
     };
     std::deque<ReloMsg> relo_buf;
-    Channel ch;
     // scratch
     std::vector<float> f_xy, f_id, f_u, f_v, f_vx, f_vy;
     std::vector<double> dt, acc, gyr, states;
 };
 
-struct BatchStep {  // what one image step of a tracker batch produced: at most one feature message per member
-    std::vector<FeatureMsg> msgs;
-    std::vector<char> has;
-    bool end = false;
-};
-
-struct BatchChannel {
-    std::mutex m;
-    std::condition_variable cv;
-    std::deque<BatchStep> q;
-    size_t depth = 2;
-    void put(BatchStep&& v) {
-        std::unique_lock<std::mutex> lk(m);
-        cv.wait(lk, [&] { return q.size() < depth; });
-        q.push_back(std::move(v));
-        cv.notify_all();
-    }
-    BatchStep get() {
-        std::unique_lock<std::mutex> lk(m);
-        cv.wait(lk, [&] { return !q.empty(); });
-        BatchStep v = std::move(q.front());
-        q.pop_front();
-        cv.notify_all();
-        return v;
-    }
+// A contiguous run of sequences with one queue between its two loops.  The library call of a step is the only thing that
+// depends on the mode: a batch lane (vr_open_batch) steps all its sequences through its batch handles in one call, a lane
+// of one sequence (vr_open) calls the sequence's own handles.
+struct Lane {
+    int first = 0, n = 1;  // sequences first .. first + n - 1 of the session
+    vt_batch* tb = nullptr;
+    ve_batch* eb = nullptr;
+    Channel ch;
 };
 
 }  // namespace
 
 struct vr_session {
-    vt_batch* tb = nullptr;  // batch mode (vr_open_batch): one tracker loop and one estimator loop for all sequences
-    ve_batch* eb = nullptr;
-    BatchChannel bch;
-    long long batch_launches = 0;
     std::vector<SeqState> seqs;
+    std::vector<Lane> lanes;
     std::string error;
     std::mutex err_m;
     std::atomic<int> status{0};
@@ -122,66 +108,110 @@ struct vr_session {
 
 namespace {
 
-// images until one publishes (or the data / the quota ends)
-void tracker_loop(vr_session* s, SeqState* q, int n_pub) {
-    for (int produced = 0; produced < n_pub && s->status.load() == 0;) {
-        FeatureMsg msg;
-        int r = 0;
-        while (r != 2 && q->cursor < q->in.n_images) {
-            const uint8_t* img = q->in.images + (size_t)q->cursor * q->in.frame_stride;
-            const double stamp = q->in.stamps[q->cursor];
-            int restart = 0;
-            r = q->in.images_on_device ? vt_node_image_device(q->trk, img, q->in.row_stride, stamp, &restart)
-                                       : vt_node_image(q->trk, img, q->in.row_stride, stamp, &restart);
-            q->cursor++;
-            if (r < 0) {
-                s->fail(r, std::string("tracker: ") + vt_last_error(q->trk));
+// Packs the feature message of the sequence's tracker (estimator_node.cpp:283-302: v = id_of_point + 0.5, feature_id = v / NUM_OF_CAM).
+int pack_message(SeqState* q, double stamp, FeatureMsg& msg) {
+    const int cap = vt_count(q->trk);
+    q->f_xy.resize(2 * (size_t)cap + 2);
+    q->f_id.resize(cap + 1);
+    q->f_u.resize(cap + 1);
+    q->f_v.resize(cap + 1);
+    q->f_vx.resize(cap + 1);
+    q->f_vy.resize(cap + 1);
+    const int n = vt_node_pack(q->trk, cap, q->f_xy.data(), q->f_id.data(), q->f_u.data(), q->f_v.data(), q->f_vx.data(), q->f_vy.data());
+    if (n < 0) return n;
+    msg.stamp = stamp;
+    msg.ids.resize(n);
+    msg.obs.resize(7 * (size_t)n);
+    for (int k = 0; k < n; k++) {
+        msg.ids[k] = (int)(q->f_id[k] + 0.5f);
+        double* o = &msg.obs[7 * (size_t)k];
+        o[0] = q->f_xy[2 * k];
+        o[1] = q->f_xy[2 * k + 1];
+        o[2] = 1.0;
+        o[3] = q->f_u[k];
+        o[4] = q->f_v[k];
+        o[5] = q->f_vx[k];
+        o[6] = q->f_vy[k];
+    }
+    return 0;
+}
+
+// img_callback for the sequences of one lane.  Every step gives each sequence that still owes published frames its next
+// image; the sequences that published hand their feature messages to the estimator loop as one Step.
+void tracker_loop(vr_session* s, Lane* L, int n_pub) {
+    SeqState* seq = &s->seqs[L->first];
+    const int S = L->n;
+    std::vector<int> produced(S, 0), active(S), results(S), restarts(S);
+    std::vector<const uint8_t*> imgs(S);
+    std::vector<double> stamps(S), h2d(S, 0.0), d2h(S, 0.0);
+    long long launches = 0;
+    while (s->status.load() == 0) {
+        bool any = false;
+        for (int k = 0; k < S; k++) {
+            const SeqState& q = seq[k];
+            active[k] = produced[k] < n_pub && q.cursor < q.in.n_images;
+            imgs[k] = active[k] ? q.in.images + (size_t)q.cursor * q.in.frame_stride : nullptr;
+            stamps[k] = active[k] ? q.in.stamps[q.cursor] : 0;
+            any = any || active[k];
+        }
+        if (!any) break;
+        int l = 0;
+        if (L->tb) {
+            const int rc = vt_batch_node_image(L->tb, active.data(), imgs.data(), seq[0].in.row_stride, stamps.data(),
+                                               seq[0].in.images_on_device, results.data(), restarts.data());
+            if (rc < 0) {
+                s->fail(rc, std::string("tracker batch: ") + vt_batch_last_error(L->tb));
                 break;
             }
-            if (r > 0) {
-                int l = 0;
-                double a = 0, b = 0;
-                vt_last_timing(q->trk, nullptr, &l);
-                vt_last_traffic(q->trk, &a, &b);
-                msg.launches += l;
-                msg.h2d += a;
-                msg.d2h += b;
+            vt_batch_last_timing(L->tb, nullptr, &l);
+        } else {
+            const SeqState& q = seq[0];
+            results[0] = q.in.images_on_device ? vt_node_image_device(q.trk, imgs[0], q.in.row_stride, stamps[0], &restarts[0])
+                                               : vt_node_image(q.trk, imgs[0], q.in.row_stride, stamps[0], &restarts[0]);
+            if (results[0] < 0) {
+                s->fail(results[0], std::string("tracker: ") + vt_last_error(q.trk));
+                break;
             }
+            if (results[0] > 0) vt_last_timing(q.trk, nullptr, &l);  // a gated-out image leaves the handle's timing stale
         }
-        if (r != 2) break;
-        const int cap = vt_count(q->trk);
-        q->f_xy.resize(2 * (size_t)cap + 2);
-        q->f_id.resize(cap + 1);
-        q->f_u.resize(cap + 1);
-        q->f_v.resize(cap + 1);
-        q->f_vx.resize(cap + 1);
-        q->f_vy.resize(cap + 1);
-        const int n = vt_node_pack(q->trk, cap, q->f_xy.data(), q->f_id.data(), q->f_u.data(), q->f_v.data(), q->f_vx.data(),
-                                   q->f_vy.data());
-        if (n < 0) {
-            s->fail(n, "tracker: vt_node_pack");
-            break;
+        launches += l;
+        Step step;
+        step.msgs.resize(S);
+        step.has.assign(S, 0);
+        bool any_msg = false;
+        for (int k = 0; k < S; k++) {
+            if (!active[k]) continue;
+            SeqState& q = seq[k];
+            q.cursor++;
+            if (results[k] > 0) {
+                double a = 0, b = 0;
+                vt_last_traffic(q.trk, &a, &b);
+                h2d[k] += a;
+                d2h[k] += b;
+            }
+            if (results[k] != 2) continue;
+            FeatureMsg& msg = step.msgs[k];
+            const int rc = pack_message(&q, stamps[k], msg);
+            if (rc < 0) {
+                s->fail(rc, L->tb ? "tracker batch: vt_node_pack" : "tracker: vt_node_pack");
+                break;
+            }
+            msg.h2d = h2d[k];
+            msg.d2h = d2h[k];
+            h2d[k] = d2h[k] = 0;
+            step.has[k] = 1;
+            produced[k]++;
+            any_msg = true;
         }
-        msg.stamp = q->in.stamps[q->cursor - 1];
-        msg.ids.resize(n);
-        msg.obs.resize(7 * (size_t)n);
-        for (int k = 0; k < n; k++) {  // estimator_node.cpp:283-302: v = id_of_point + 0.5, feature_id = v / NUM_OF_CAM
-            msg.ids[k] = (int)(q->f_id[k] + 0.5f);
-            double* o = &msg.obs[7 * (size_t)k];
-            o[0] = q->f_xy[2 * k];
-            o[1] = q->f_xy[2 * k + 1];
-            o[2] = 1.0;
-            o[3] = q->f_u[k];
-            o[4] = q->f_v[k];
-            o[5] = q->f_vx[k];
-            o[6] = q->f_vy[k];
+        if (any_msg) {
+            step.launches = launches;
+            launches = 0;
+            L->ch.put(std::move(step));
         }
-        q->ch.put(std::move(msg));
-        produced++;
     }
-    FeatureMsg fin;
+    Step fin;
     fin.end = true;
-    q->ch.put(std::move(fin));
+    L->ch.put(std::move(fin));
 }
 
 void imu_one(SeqState* q, int k, double img_t) {
@@ -241,170 +271,31 @@ void apply_relo(SeqState* q, double now) {
     for (size_t k = 0; k < n_pop; k++) q->relo_buf.pop_front();
 }
 
-void estimator_loop(vr_session* s, SeqState* q) {
-    for (;;) {
-        FeatureMsg msg = q->ch.get();
-        if (msg.end) break;
-        if (s->status.load() != 0) continue;  // keep draining so that the producer can finish
-        long long launches = msg.launches;
-        double h2d = msg.h2d, d2h = msg.d2h;
-        if (q->first_msg) {
-            q->first_msg = false;
-        } else {
-            double td = 0;  // img_t = stamp + estimator.td in getMeasurements and process() (estimator_node.cpp:106-126, 232-265)
-            ve_get_states(q->est, q->states.data(), &td);
-            collect_imu(q, msg.stamp + td);
-            int rc = q->dt.empty() ? 0 : ve_process_imu_batch(q->est, (int)q->dt.size(), q->dt.data(), q->acc.data(), q->gyr.data());
-            apply_relo(q, msg.stamp);
-            if (rc == 0) rc = ve_process_image(q->est, (int)msg.ids.size(), msg.ids.data(), msg.obs.data(), msg.stamp);
-            if (rc < 0) {
-                s->fail(rc, std::string("estimator: ") + ve_last_error(q->est));
-                continue;
-            }
-            int l = 0;
-            double a = 0, b = 0;
-            ve_last_timing(q->est, nullptr, &l);
-            ve_last_traffic(q->est, &a, &b);
-            launches += l;
-            h2d += a;
-            d2h += b;
-        }
-        q->frames++;
-        q->launches += launches;
-        q->h2d += h2d;
-        q->d2h += d2h;
-        int info[10];
-        double costs[2];
-        if (ve_info(q->est, info, costs) == 0 && info[0] == 1) {
-            ve_get_states(q->est, q->states.data(), nullptr);
-            const double* newest = &q->states[16 * (size_t)info[1]];  // frame_count == WINDOW_SIZE: the newest frame
-            q->traj_t.push_back(msg.stamp);
-            q->traj_p.insert(q->traj_p.end(), newest, newest + 3);
-        }
-    }
-}
-
-// Packs the feature message of tracker handle trk (estimator_node.cpp:283-302: v = id_of_point + 0.5, feature_id = v / NUM_OF_CAM).
-int pack_message(SeqState* q, vt_tracker* trk, double stamp, FeatureMsg& msg) {
-    const int cap = vt_count(trk);
-    q->f_xy.resize(2 * (size_t)cap + 2);
-    q->f_id.resize(cap + 1);
-    q->f_u.resize(cap + 1);
-    q->f_v.resize(cap + 1);
-    q->f_vx.resize(cap + 1);
-    q->f_vy.resize(cap + 1);
-    const int n = vt_node_pack(trk, cap, q->f_xy.data(), q->f_id.data(), q->f_u.data(), q->f_v.data(), q->f_vx.data(), q->f_vy.data());
-    if (n < 0) return n;
-    msg.stamp = stamp;
-    msg.ids.resize(n);
-    msg.obs.resize(7 * (size_t)n);
-    for (int k = 0; k < n; k++) {
-        msg.ids[k] = (int)(q->f_id[k] + 0.5f);
-        double* o = &msg.obs[7 * (size_t)k];
-        o[0] = q->f_xy[2 * k];
-        o[1] = q->f_xy[2 * k + 1];
-        o[2] = 1.0;
-        o[3] = q->f_u[k];
-        o[4] = q->f_v[k];
-        o[5] = q->f_vx[k];
-        o[6] = q->f_vy[k];
-    }
-    return 0;
-}
-
-// Batch mode, tracker side: every sequence that still owes published frames consumes its next image in the same
-// vt_batch_node_image call; the members that published hand their messages to the estimator loop as one BatchStep.
-void tracker_batch_loop(vr_session* s, int n_pub) {
-    const int S = (int)s->seqs.size();
-    std::vector<int> produced(S, 0), active(S), results(S), restarts(S);
-    std::vector<const uint8_t*> imgs(S);
-    std::vector<double> stamps(S);
-    std::vector<double> acc_h2d(S, 0.0), acc_d2h(S, 0.0);
-    long long acc_launches = 0;
-    while (s->status.load() == 0) {
-        bool any = false;
-        for (int k = 0; k < S; k++) {
-            SeqState& q = s->seqs[k];
-            active[k] = produced[k] < n_pub && q.cursor < q.in.n_images;
-            imgs[k] = nullptr;
-            stamps[k] = 0;
-            if (!active[k]) continue;
-            any = true;
-            imgs[k] = q.in.images + (size_t)q.cursor * q.in.frame_stride;
-            stamps[k] = q.in.stamps[q.cursor];
-        }
-        if (!any) break;
-        const vr_sequence& in0 = s->seqs[0].in;
-        const int rc = vt_batch_node_image(s->tb, active.data(), imgs.data(), in0.row_stride, stamps.data(), in0.images_on_device,
-                                           results.data(), restarts.data());
-        if (rc < 0) {
-            s->fail(rc, std::string("tracker batch: ") + vt_batch_last_error(s->tb));
-            break;
-        }
-        int l = 0;
-        vt_batch_last_timing(s->tb, nullptr, &l);
-        acc_launches += l;
-        BatchStep step;
-        step.msgs.resize(S);
-        step.has.assign(S, 0);
-        bool any_msg = false;
-        for (int k = 0; k < S; k++) {
-            if (!active[k]) continue;
-            SeqState& q = s->seqs[k];
-            q.cursor++;
-            if (results[k] > 0) {
-                double a = 0, b = 0;
-                vt_last_traffic(q.trk, &a, &b);
-                acc_h2d[k] += a;
-                acc_d2h[k] += b;
-            }
-            if (results[k] != 2) continue;
-            FeatureMsg& msg = step.msgs[k];
-            const int prc = pack_message(&q, q.trk, stamps[k], msg);
-            if (prc < 0) {
-                s->fail(prc, "tracker batch: vt_node_pack");
-                break;
-            }
-            msg.h2d = acc_h2d[k];
-            msg.d2h = acc_d2h[k];
-            acc_h2d[k] = acc_d2h[k] = 0;
-            step.has[k] = 1;
-            produced[k]++;
-            any_msg = true;
-        }
-        if (any_msg) {
-            step.msgs[0].launches += acc_launches;  // batch launches are not attributable to a member: carried on member 0's slot
-            acc_launches = 0;
-            s->bch.put(std::move(step));
-        }
-    }
-    BatchStep fin;
-    fin.end = true;
-    s->bch.put(std::move(fin));
-}
-
-// Batch mode, estimator side: IMU selection per member, then ONE ve_batch_process_image for all members with a message.
-void estimator_batch_loop(vr_session* s) {
-    const int S = (int)s->seqs.size();
+// process() for the sequences of one lane.  Per sequence with a message: the first message is dropped, the others get
+// their IMU samples up to stamp + td and their relocalisation message.  An IMU failure ends the step there.  Then one
+// processImage call serves the whole step, and every sequence it processed adds a trajectory row.
+void estimator_loop(vr_session* s, Lane* L) {
+    SeqState* seq = &s->seqs[L->first];
+    const int S = L->n;
     std::vector<int> active(S), n(S), status(S);
     std::vector<const int*> ids(S);
     std::vector<const double*> obs(S);
     std::vector<double> stamps(S);
     for (;;) {
-        BatchStep step = s->bch.get();
+        Step step = L->ch.get();
         if (step.end) break;
         if (s->status.load() != 0) continue;  // keep draining so that the producer can finish
+        seq[0].launches += step.launches;
         bool any = false;
-        s->batch_launches += step.msgs[0].launches;
         for (int k = 0; k < S; k++) {
-            SeqState& q = s->seqs[k];
             active[k] = 0;
             n[k] = 0;
             ids[k] = nullptr;
             obs[k] = nullptr;
             stamps[k] = 0;
             if (!step.has[k]) continue;
-            FeatureMsg& msg = step.msgs[k];
+            SeqState& q = seq[k];
+            const FeatureMsg& msg = step.msgs[k];
             q.h2d += msg.h2d;
             q.d2h += msg.d2h;
             if (q.first_msg) {  // estimator_node.cpp:167-172
@@ -412,7 +303,7 @@ void estimator_batch_loop(vr_session* s) {
                 q.frames++;
                 continue;
             }
-            double td = 0;
+            double td = 0;  // img_t = stamp + estimator.td in getMeasurements and process() (estimator_node.cpp:106-126, 232-265)
             ve_get_states(q.est, q.states.data(), &td);
             collect_imu(&q, msg.stamp + td);
             const int rc = q.dt.empty() ? 0 : ve_process_imu_batch(q.est, (int)q.dt.size(), q.dt.data(), q.acc.data(), q.gyr.data());
@@ -429,17 +320,21 @@ void estimator_batch_loop(vr_session* s) {
             any = true;
         }
         if (s->status.load() != 0 || !any) continue;
-        const int rc = ve_batch_process_image(s->eb, active.data(), n.data(), ids.data(), obs.data(), stamps.data(), status.data());
-        if (rc < 0) {
-            s->fail(rc, std::string("estimator batch: ") + ve_batch_last_error(s->eb));
-            continue;
+        int rc, l = 0;
+        if (L->eb) {
+            rc = ve_batch_process_image(L->eb, active.data(), n.data(), ids.data(), obs.data(), stamps.data(), status.data());
+            if (rc < 0) s->fail(rc, std::string("estimator batch: ") + ve_batch_last_error(L->eb));
+            else ve_batch_last_timing(L->eb, nullptr, &l);
+        } else {
+            rc = ve_process_image(seq[0].est, n[0], ids[0], obs[0], stamps[0]);
+            if (rc < 0) s->fail(rc, std::string("estimator: ") + ve_last_error(seq[0].est));
+            else ve_last_timing(seq[0].est, nullptr, &l);
         }
-        int l = 0;
-        ve_batch_last_timing(s->eb, nullptr, &l);
-        s->batch_launches += l;
+        if (rc < 0) continue;
+        seq[0].launches += l;
         for (int k = 0; k < S; k++) {
             if (!active[k]) continue;
-            SeqState& q = s->seqs[k];
+            SeqState& q = seq[k];
             double a = 0, b = 0;
             ve_last_traffic(q.est, &a, &b);
             q.h2d += a;
@@ -449,12 +344,39 @@ void estimator_batch_loop(vr_session* s) {
             double costs[2];
             if (ve_info(q.est, info, costs) == 0 && info[0] == 1) {
                 ve_get_states(q.est, q.states.data(), nullptr);
-                const double* newest = &q.states[16 * (size_t)info[1]];
+                const double* newest = &q.states[16 * (size_t)info[1]];  // frame_count == WINDOW_SIZE: the newest frame
                 q.traj_t.push_back(stamps[k]);
                 q.traj_p.insert(q.traj_p.end(), newest, newest + 3);
             }
         }
     }
+}
+
+// The argument checks and the set-up vr_open and vr_open_batch share: a SeqState per sequence, and one lane of all the
+// sequences for a batch (tb, eb) or a lane per sequence.
+int open_session(int n_seq, vt_tracker* const* trk, ve_estimator* const* est, const vr_sequence* seqs, vt_batch* tb, ve_batch* eb,
+                 vr_session** out) {
+    for (int k = 0; k < n_seq; k++)
+        if (!trk[k] || !est[k] || !seqs[k].images || !seqs[k].stamps || (seqs[k].n_imu > 0 && !seqs[k].imu_t)) return -1;
+    auto* s = new vr_session;
+    s->seqs = std::vector<SeqState>(n_seq);
+    for (int k = 0; k < n_seq; k++) {
+        SeqState& q = s->seqs[k];
+        q.trk = trk[k];
+        q.est = est[k];
+        q.in = seqs[k];
+        q.states.assign(16 * (size_t)(ve_window_size(est[k]) + 1), 0.0);
+    }
+    s->lanes = std::vector<Lane>(tb ? 1 : n_seq);
+    for (size_t l = 0; l < s->lanes.size(); l++) {
+        Lane& L = s->lanes[l];
+        L.first = (int)l;
+        L.n = tb ? n_seq : 1;
+        L.tb = tb;
+        L.eb = eb;
+    }
+    *out = s;
+    return 0;
 }
 
 }  // namespace
@@ -465,43 +387,19 @@ int vr_open_batch(vt_batch* trackers, ve_batch* estimators, const vr_sequence* s
     if (!trackers || !estimators || !seqs || !out) return -1;
     const int n_seq = vt_batch_size(trackers);
     if (n_seq <= 0 || n_seq != ve_batch_size(estimators)) return -1;
-    auto* s = new vr_session;
-    s->tb = trackers;
-    s->eb = estimators;
-    s->seqs = std::vector<SeqState>(n_seq);
+    std::vector<vt_tracker*> trk(n_seq);
+    std::vector<ve_estimator*> est(n_seq);
     for (int k = 0; k < n_seq; k++) {
-        SeqState& q = s->seqs[k];
-        if (!seqs[k].images || !seqs[k].stamps || (seqs[k].n_imu > 0 && !seqs[k].imu_t) || seqs[k].row_stride != seqs[0].row_stride ||
-            seqs[k].images_on_device != seqs[0].images_on_device) {
-            delete s;
-            return -1;
-        }
-        q.trk = vt_batch_member(trackers, k);
-        q.est = ve_batch_member(estimators, k);
-        q.in = seqs[k];
-        q.states.assign(16 * 65, 0.0);
+        if (seqs[k].row_stride != seqs[0].row_stride || seqs[k].images_on_device != seqs[0].images_on_device) return -1;
+        trk[k] = vt_batch_member(trackers, k);
+        est[k] = ve_batch_member(estimators, k);
     }
-    *out = s;
-    return 0;
+    return open_session(n_seq, trk.data(), est.data(), seqs, trackers, estimators, out);
 }
 
 int vr_open(int n_seq, vt_tracker* const* trackers, ve_estimator* const* estimators, const vr_sequence* seqs, vr_session** out) {
     if (n_seq <= 0 || !trackers || !estimators || !seqs || !out) return -1;
-    auto* s = new vr_session;
-    s->seqs = std::vector<SeqState>(n_seq);
-    for (int k = 0; k < n_seq; k++) {
-        SeqState& q = s->seqs[k];
-        if (!trackers[k] || !estimators[k] || !seqs[k].images || !seqs[k].stamps || (seqs[k].n_imu > 0 && !seqs[k].imu_t)) {
-            delete s;
-            return -1;
-        }
-        q.trk = trackers[k];
-        q.est = estimators[k];
-        q.in = seqs[k];
-        q.states.assign(16 * 65, 0.0);  // window_size + 1 <= 65 rows
-    }
-    *out = s;
-    return 0;
+    return open_session(n_seq, trackers, estimators, seqs, nullptr, nullptr, out);
 }
 
 void vr_close(vr_session* s) { delete s; }
@@ -514,14 +412,10 @@ int vr_advance(vr_session* s, int n_pub) {
     std::vector<int> before(s->seqs.size());
     std::vector<std::thread> threads;
     for (size_t k = 0; k < s->seqs.size(); k++) before[k] = s->seqs[k].frames;
-    if (s->tb) {
-        threads.emplace_back(tracker_batch_loop, s, n_pub);
-        threads.emplace_back(estimator_batch_loop, s);
-    } else
-        for (size_t k = 0; k < s->seqs.size(); k++) {
-            threads.emplace_back(tracker_loop, s, &s->seqs[k], n_pub);
-            threads.emplace_back(estimator_loop, s, &s->seqs[k]);
-        }
+    for (Lane& L : s->lanes) {
+        threads.emplace_back(tracker_loop, s, &L, n_pub);
+        threads.emplace_back(estimator_loop, s, &L);
+    }
     for (auto& t : threads) t.join();
     if (s->status.load() != 0) return s->status.load();
     int total = 0;
@@ -636,10 +530,10 @@ int vr_prop_update_from_estimator(vr_propagator* p, const ve_estimator* e, doubl
     if (!p || !e) return -1;
     int info[10];
     if (ve_info(e, info, nullptr) != 0) return -1;
-    std::vector<double> st(16 * 65, 0.0);
+    const int W = ve_window_size(e);
+    std::vector<double> st(16 * (size_t)(W + 1), 0.0);
     double imu0[9];
     if (ve_get_states(e, st.data(), nullptr) != 0 || ve_get_latest_imu(e, imu0, imu0 + 3, imu0 + 6) != 0) return -1;
-    const int W = ve_window_size(e);
     const double* s = &st[16 * (size_t)W];
     return vr_prop_update(p, current_time, s, s + 3, s + 7, s + 10, s + 13, imu0, imu0 + 3, imu0 + 6, n, t, acc, gyr);
 }
@@ -684,12 +578,8 @@ int vr_decode_relo_message(int n, const float* xyz, const float* channel0_values
     const float* c = channel0_values8;
     for (int k = 0; k < 3; k++) relo_t3[k] = c[k];
     // Quaterniond relo_q(values[3], values[4], values[5], values[6]) = (w, x, y, z); toRotationMatrix() does not normalise
-    const double w = c[3], x = c[4], y = c[5], z = c[6];
-    const double tx = 2 * x, ty = 2 * y, tz = 2 * z, twx = tx * w, twy = ty * w, twz = tz * w;
-    const double txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
-    relo_r9[0] = 1 - (tyy + tzz); relo_r9[1] = txy - twz; relo_r9[2] = txz + twy;
-    relo_r9[3] = txy + twz; relo_r9[4] = 1 - (txx + tzz); relo_r9[5] = tyz - twx;
-    relo_r9[6] = txz - twy; relo_r9[7] = tyz + twx; relo_r9[8] = 1 - (txx + tyy);
+    const hm::Mat3 R = hm::Quat(c[3], c[4], c[5], c[6]).R();
+    std::memcpy(relo_r9, R.m, sizeof(R.m));
     if (frame_index) *frame_index = (int)c[7];
     return n;
 }
@@ -715,7 +605,7 @@ int vr_stats(const vr_session* s, int seq, int* frames, long long* launches, dou
     if (!s || seq < 0 || seq >= (int)s->seqs.size()) return -1;
     const SeqState& q = s->seqs[seq];
     if (frames) *frames = q.frames;
-    if (launches) *launches = s->tb ? (seq == 0 ? s->batch_launches : 0) : q.launches;
+    if (launches) *launches = q.launches;
     if (h2d_bytes) *h2d_bytes = q.h2d;
     if (d2h_bytes) *d2h_bytes = q.d2h;
     return 0;
