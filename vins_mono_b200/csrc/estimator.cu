@@ -12,26 +12,22 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <cmath>
-#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <memory>
-#include <mutex>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "ba_kernels.h"
 #include "ba_layout.h"
+#include "batch_host.h"
 #include "cuda_check.h"
 #include "host_math.h"
-#include <array>
-
 #include "hostpool.h"
 #include "initial.h"
 #include "vinsb200/estimator.h"
@@ -69,12 +65,9 @@ enum FrameStage { STAGE_DONE = 0, STAGE_INIT_SOLVE = 1, STAGE_RUN_SOLVE = 2 };
 
 }  // namespace
 
-struct ve_estimator {
+struct ve_estimator : vb::MemberBase<ve_batch> {
     ve_config cfg{};
-    std::string err;
     int W = 10;
-    ve_batch* batch = nullptr;
-    int member = 0;
     // ---- Estimator state (estimator.h:65-115)
     int solver_flag = 0;           // INITIAL = 0, NON_LINEAR = 1
     int marginalization_flag = 0;  // MARGIN_OLD = 0, MARGIN_SECOND_NEW = 1
@@ -156,12 +149,8 @@ struct ve_estimator {
     vb::DeviceArray<double> d_marg;        // Am | bm | Araw | graw | Wglobal
 };
 
-struct ve_batch {
+struct ve_batch : vb::BatchBase<ve_estimator> {
     ve_config cfg{};
-    int S = 0;
-    bool standalone = false;  // created by ve_create: destroyed with its only member
-    std::vector<ve_estimator*> members;
-    std::string err;
     // Launch groups: the members are split into G contiguous groups, each with its own streams, events and arena slices.
     // Every group runs the same launch chain over its members; the chains of different groups overlap on the GPU (the
     // single-CTA-per-member solvers of one group leave most SMs to the wide kernels of another).
@@ -1182,7 +1171,7 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
     }
     b->last_launches = 0;
     b->pool->run(S, [&](int k) {
-        ve_estimator* e = b->members[k];
+        ve_estimator* e = b->members[k].get();
         vb::BaSeq& q = b->h_seq[k];
         q.active = q.do_marg = q.n_jobs = 0;
         q.sqrt_mask = 0;
@@ -1195,7 +1184,6 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
     });
     const double t_prepare = since(t0);
     const auto t1 = std::chrono::steady_clock::now();
-    int rc = VE_OK;
     b->marg_timing_valid = false;
     b->last_ms[0] = b->last_ms[1] = b->last_ms[2] = b->last_ms[3] = 0;
     for (int g = 0; g < b->G; g++) {  // enqueue every group's chain; nothing is waited for inside this loop
@@ -1273,16 +1261,11 @@ int batch_process(ve_batch* b, const FrameMsg* msgs, int* status_out) {
     }
     const double t_wait = since(t2);
     const auto t3 = std::chrono::steady_clock::now();
-    b->pool->run(S, [&](int k) { finish_frame(b->members[k]); });
+    b->pool->run(S, [&](int k) { finish_frame(b->members[k].get()); });
     if (trace) std::fprintf(stderr, "[ve_batch] prepare %.3f launch %.3f wait %.3f finish %.3f ms (S=%d)\n", t_prepare, t_launch, t_wait, since(t3), S);
-    for (int k = 0; k < S; k++) {
-        if (status_out) status_out[k] = b->members[k]->status;
-        if (b->members[k]->status != VE_OK && rc == VE_OK) {
-            rc = b->members[k]->status;
-            b->err = "member " + std::to_string(k) + ": " + b->members[k]->err;
-        }
-    }
-    return rc;
+    if (status_out)
+        for (int k = 0; k < S; k++) status_out[k] = b->members[k]->status;
+    return vb::roll_up(b, VE_OK);
 }
 
 int config_valid(const ve_config* cfg) {
@@ -1330,7 +1313,7 @@ int create_member(ve_batch* b, int k) {
     VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_vec.alloc(vb::ba_vec_layout(e->D, e->Lmax).total));
     VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_work.alloc(vb::ba_work_layout(e->D, e->Lmax).total));
     VB_CUDA_CHECK(b, VE_ERR_CUDA, e->d_marg.alloc(vb::ba_marg_layout(e->nmax, e->Lmax).total));
-    b->members.push_back(e.release());
+    b->members.push_back(std::move(e));
     return VE_OK;
 }
 
@@ -1369,7 +1352,7 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
         const int rc = create_member(b.get(), k);
         if (rc) return rc;
     }
-    const ve_estimator* e0 = b->members[0];
+    const ve_estimator* e0 = b->members[0].get();
     const int W = cfg->window_size, F = W + 1;
     const size_t per_in = vb::ba_in_layout_max(W, e0->Lmax, e0->Mmax).total;  // one member's input block at full capacity
     // a batch rarely has every member at capacity: size the arenas for the full capacity of 8 members or a quarter of
@@ -1400,23 +1383,21 @@ int ve_batch_create(const ve_config* cfg, int n, ve_batch** out) {
 }
 
 void ve_batch_destroy(ve_batch* b) {
-    if (!b) return;
-    cudaSetDevice(b->cfg.device);
-    for (int g = 0; b->groups && g < b->G; g++) {
-        if (b->groups[g].stream) cudaStreamSynchronize(b->groups[g].stream);
-        if (b->groups[g].copy_stream) cudaStreamSynchronize(b->groups[g].copy_stream);
-    }
-    b->pool.reset();
-    for (auto* e : b->members) delete e;
-    delete b;
+    vb::destroy_batch(b, [b] {
+        for (int g = 0; b->groups && g < b->G; g++) {
+            if (b->groups[g].stream) cudaStreamSynchronize(b->groups[g].stream);
+            if (b->groups[g].copy_stream) cudaStreamSynchronize(b->groups[g].copy_stream);
+        }
+        b->pool.reset();
+    });
 }
 
-int ve_batch_size(const ve_batch* b) { return b ? b->S : VE_ERR_INVALID; }
+int ve_batch_size(const ve_batch* b) { return vb::batch_size(b, VE_ERR_INVALID); }
 int ve_batch_groups(const ve_batch* b) { return b ? b->G : VE_ERR_INVALID; }
 
-ve_estimator* ve_batch_member(ve_batch* b, int k) { return (b && k >= 0 && k < b->S) ? b->members[k] : nullptr; }
+ve_estimator* ve_batch_member(ve_batch* b, int k) { return vb::batch_member(b, k); }
 
-const char* ve_batch_last_error(const ve_batch* b) { return b ? b->err.c_str() : "null batch"; }
+const char* ve_batch_last_error(const ve_batch* b) { return vb::batch_last_error(b); }
 
 int ve_batch_process_image(ve_batch* b, const int* active, const int* n, const int* const* ids, const double* const* xyz_uv_vel,
                            const double* stamps, int* status) {
@@ -1448,21 +1429,9 @@ int ve_batch_last_timing(const ve_batch* cb, float* ms4, int* launches) {
     return VE_OK;
 }
 
-int ve_batch_set_profile(ve_batch* b, int on) {
-    if (!b) return VE_ERR_INVALID;
-    VB_CUDA_CHECK(b, VE_ERR_CUDA, cudaSetDevice(b->cfg.device));
-    b->prof.enable(on != 0);
-    return VE_OK;
-}
+int ve_batch_set_profile(ve_batch* b, int on) { return vb::set_profile(b, on, VE_ERR_INVALID, VE_ERR_CUDA); }
 
-int ve_batch_kernel_times(const ve_batch* b, double* ms8, int* count8) {
-    if (!b) return VE_ERR_INVALID;
-    for (int k = 0; k < 8; k++) {
-        if (ms8) ms8[k] = b->prof.ms[k];
-        if (count8) count8[k] = b->prof.count[k];
-    }
-    return VE_OK;
-}
+int ve_batch_kernel_times(const ve_batch* b, double* ms8, int* count8) { return vb::kernel_times(b, ms8, count8, 8, VE_ERR_INVALID); }
 
 int ve_batch_sync(ve_batch* b) {
     if (!b) return VE_ERR_INVALID;
@@ -1471,26 +1440,11 @@ int ve_batch_sync(ve_batch* b) {
     return VE_OK;
 }
 
-int ve_create(const ve_config* cfg, ve_estimator** out) {
-    if (!cfg || !out) return VE_ERR_INVALID;
-    *out = nullptr;
-    ve_batch* b = nullptr;
-    const int rc = ve_batch_create(cfg, 1, &b);
-    if (rc) return rc;
-    b->standalone = true;
-    *out = b->members[0];
-    return VE_OK;
-}
+int ve_create(const ve_config* cfg, ve_estimator** out) { return vb::create_standalone(ve_batch_create, cfg, out, VE_ERR_INVALID); }
 
-void ve_destroy(ve_estimator* e) {
-    if (!e) return;
-    if (e->batch && e->batch->standalone) ve_batch_destroy(e->batch);  // members of an explicit batch die with the batch
-}
+void ve_destroy(ve_estimator* e) { vb::destroy_standalone(e, ve_batch_destroy); }
 
-const char* ve_last_error(const ve_estimator* e) {
-    if (!e) return "null handle";
-    return e->err.empty() && e->batch ? e->batch->err.c_str() : e->err.c_str();
-}
+const char* ve_last_error(const ve_estimator* e) { return vb::last_error(e); }
 
 int ve_clear_state(ve_estimator* e) {
     if (!e) return VE_ERR_INVALID;
@@ -1531,14 +1485,11 @@ int ve_process_imu_batch(ve_estimator* e, int n, const double* dt, const double*
 
 int ve_process_image(ve_estimator* e, int n, const int* ids, const double* xyz_uv_vel, double stamp) {
     if (!e || n < 0 || (n && (!ids || !xyz_uv_vel))) return VE_ERR_INVALID;
-    ve_batch* b = e->batch;
-    if (!b->standalone) {
-        e->err = "ve_process_image on a member of a batch: use ve_batch_process_image";
-        return VE_ERR_INVALID;
-    }
+    if (const int rc = vb::refuse_member(e, VE_ERR_INVALID, "ve_process_image on a member of a batch: use ve_batch_process_image"))
+        return rc;
     e->err.clear();
     FrameMsg m{1, n, ids, xyz_uv_vel, stamp};
-    return batch_process(b, &m, nullptr);
+    return batch_process(e->batch, &m, nullptr);
 }
 
 int ve_get_states(const ve_estimator* e, double* out, double* td) {

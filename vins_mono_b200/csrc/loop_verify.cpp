@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "batch_host.h"
 #include "camera_lift.h"
 #include "cuda_check.h"
 #include "host_math.h"
@@ -359,55 +360,45 @@ int vp_batch_loop_enable(vp_batch* b, const vp_loop_config* cfg) { return vp_bat
 
 int vp_loop_enable_camera(vp_graph* g, const vp_loop_config* cfg, int camera_model, double xi) {
     if (!g) return VP_ERR_INVALID;
-    int member = 0, device = 0;
-    bool standalone = false;
-    vp_batch* b = vb::pg_owner(g, &member, &standalone);
-    if (!standalone) {
-        *vb::pg_error(g) = "vp_loop_enable: a batch member is enabled through vp_batch_loop_enable";
-        return VP_ERR_INVALID;
-    }
-    const int cap = vb::pg_capacity(b, &device);
-    return enable(vb::pg_loop_state(b), cfg, camera_model, xi, 1, cap, device, vb::pg_error(g));
+    if (const int rc = vb::refuse_member(g, VP_ERR_INVALID, "vp_loop_enable: a batch member is enabled through vp_batch_loop_enable"))
+        return rc;
+    vp_batch* b = g->batch;
+    return enable(&b->lv, cfg, camera_model, xi, 1, b->cfg.max_keyframes, b->cfg.device, &g->err);
 }
 
 int vp_batch_loop_enable_camera(vp_batch* b, const vp_loop_config* cfg, int camera_model, double xi) {
     if (!b) return VP_ERR_INVALID;
-    int device = 0;
-    const int cap = vb::pg_capacity(b, &device);
-    return enable(vb::pg_loop_state(b), cfg, camera_model, xi, vp_batch_size(b), cap, device, vb::pg_batch_error(b));
+    return enable(&b->lv, cfg, camera_model, xi, b->S, b->cfg.max_keyframes, b->cfg.device, &b->err);
 }
 
 int vp_attach_keyframe(vp_graph* g, int index, const double* vio_P3, const double* vio_Qwxyz, const uint8_t* img, size_t row_stride,
                        int n, const float* point_3d, const float* point_uv, const float* point_norm, const double* point_id,
                        int* n_corners) {
     if (!g) return VP_ERR_INVALID;
-    int member = 0;
-    bool standalone = false;
-    LvState* s = *vb::pg_loop_state(vb::pg_owner(g, &member, &standalone));
+    LvState* s = g->batch->lv;
     if (!s) {
-        *vb::pg_error(g) = "vp_attach_keyframe: loop verification is not enabled";
+        g->err = "vp_attach_keyframe: loop verification is not enabled";
         return VP_ERR_INVALID;
     }
-    return attach(s, member, index, vio_P3, vio_Qwxyz, img, row_stride, n, point_3d, point_uv, point_norm, point_id, n_corners,
-                  vb::pg_error(g));
+    return attach(s, g->member, index, vio_P3, vio_Qwxyz, img, row_stride, n, point_3d, point_uv, point_norm, point_id, n_corners,
+                  &g->err);
 }
 
 int vp_find_connection(vp_graph* g, int cur, int old, vp_loop_result* r, int cap, double* match_xyid) {
     if (!g || !r || (match_xyid && cap < 0)) return VP_ERR_INVALID;
-    int member = 0;
-    bool standalone = false;
-    LvState* s = *vb::pg_loop_state(vb::pg_owner(g, &member, &standalone));
+    LvState* s = g->batch->lv;
     if (!s) {
-        *vb::pg_error(g) = "vp_find_connection: loop verification is not enabled";
+        g->err = "vp_find_connection: loop verification is not enabled";
         return VP_ERR_INVALID;
     }
+    const int member = g->member;
     std::vector<int> c(s->S, -1), o(s->S, -1);
     std::vector<vp_loop_result> rr(s->S);
     c[member] = cur < 0 ? s->cap_kf : cur;  // a negative index is an argument error here, not "skip"
     o[member] = old;
     std::vector<double> list;
     if (match_xyid) list.assign((size_t)3 * cap * s->S, 0.0);
-    const int rc = connect(s, c.data(), o.data(), rr.data(), cap, match_xyid ? list.data() : nullptr, nullptr, vb::pg_error(g));
+    const int rc = connect(s, c.data(), o.data(), rr.data(), cap, match_xyid ? list.data() : nullptr, nullptr, &g->err);
     if (rc) return rc;
     *r = rr[member];
     if (match_xyid && r->n_points) std::memcpy(match_xyid, list.data() + 3 * (size_t)cap * member, 3 * sizeof(double) * r->n_points);
@@ -416,27 +407,25 @@ int vp_find_connection(vp_graph* g, int cur, int old, vp_loop_result* r, int cap
 
 int vp_batch_find_connection(vp_batch* b, const int* cur, const int* old, vp_loop_result* r, int cap, double* match_xyid, int* status) {
     if (!b || !cur || !old || !r || (match_xyid && cap < 0)) return VP_ERR_INVALID;
-    LvState* s = *vb::pg_loop_state(b);
+    LvState* s = b->lv;
     if (!s) {
-        *vb::pg_batch_error(b) = "vp_batch_find_connection: loop verification is not enabled";
+        b->err = "vp_batch_find_connection: loop verification is not enabled";
         return VP_ERR_INVALID;
     }
-    return connect(s, cur, old, r, cap, match_xyid, status, vb::pg_batch_error(b));
+    return connect(s, cur, old, r, cap, match_xyid, status, &b->err);
 }
 
 int vp_loop_last_timing(vp_graph* g, float* ms6) {
     if (!g || !ms6) return VP_ERR_INVALID;
-    int member = 0;
-    bool standalone = false;
-    LvState* s = *vb::pg_loop_state(vb::pg_owner(g, &member, &standalone));
+    const LvState* s = g->batch->lv;
     if (!s) return VP_ERR_INVALID;
     std::memcpy(ms6, s->ms, sizeof(s->ms));
     return 0;
 }
 
 int vp_batch_loop_last_timing(vp_batch* b, float* ms6) {
-    if (!b || !ms6 || !*vb::pg_loop_state(b)) return VP_ERR_INVALID;
-    std::memcpy(ms6, (*vb::pg_loop_state(b))->ms, sizeof(float) * 6);
+    if (!b || !ms6 || !b->lv) return VP_ERR_INVALID;
+    std::memcpy(ms6, b->lv->ms, sizeof(float) * 6);
     return 0;
 }
 

@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "batch_host.h"
 #include "cuda_check.h"
 #include "host_math.h"
 #include "pg_host.h"
@@ -22,79 +23,17 @@
 using hm::Mat3;
 using hm::Quat;
 using hm::Vec3;
+using KeyFrame = vb::PgKeyFrame;
 
 namespace {
 
 constexpr int PG_MAX_ITERATIONS = 5;  // options.max_num_iterations, pose_graph.cpp:437
-
-struct KeyFrame {
-    double stamp = 0;
-    Vec3 vio_P, P;
-    Mat3 vio_R, R;
-    int seq = 0;
-    bool has_loop = false;
-    int loop_index = -1;
-    double loop_info[8] = {};
-};
 
 bool loop_gate(const double* li) {  // keyframe.cpp:480, :573
     return std::fabs(li[7]) < 30.0 && Vec3(li[0], li[1], li[2]).norm() < 20.0;
 }
 
 Mat3 yaw_R(double yaw) { return hm::ypr2R(Vec3(yaw, 0, 0)); }
-
-}  // namespace
-
-struct vp_graph {
-    vp_batch* owner = nullptr;
-    int member = 0;
-    bool standalone = false;
-    vp_config cfg{};
-    std::string err;
-    std::vector<KeyFrame> kfs;
-    int sequence = 1;      // the node's sequence counter (pose_graph_node.cpp:69-72)
-    int sequence_cnt = 0;  // PoseGraph::sequence_cnt
-    std::vector<int> sequence_loop{0};
-    Mat3 w_r_vio, r_drift;
-    Vec3 w_t_vio, t_drift;
-    double yaw_drift = 0;
-    int earliest_loop_index = -1, pending = -1, n_loops = 0, n_opt = 0;
-    int n_map = 0;  // key frames 0 .. n_map - 1 came from vp_load: sequence 0, constant in every optimisation
-    // the optimisation in flight (enqueued, not collected): its range, the key frames it packed (global index by local
-    // index), the pitch / roll it used, its output once copied
-    bool inflight = false, ready = false;
-    int inf_first = 0, inf_cur = 0, inf_D = 0;
-    std::vector<int> inf_map;
-    std::vector<double> inf_pr, inf_out;
-    int last_info[4] = {0, 0, 0, 0};
-    double last_cost[2] = {0, 0};
-    float last_ms = 0;
-    int last_launches = 0;
-};
-
-struct vp_batch {
-    vp_config cfg{};
-    int S = 0;
-    int cap_anchors = 0;  // free loop anchors an optimised range may hold (vp_config::max_anchors, 0 = PG_MAX_ANCHORS)
-    std::string err;
-    std::vector<vp_graph*> members;
-    vb::PinnedArray<char> h_in;
-    vb::DeviceArray<char> d_in;
-    vb::PinnedArray<double> h_out;
-    vb::DeviceArray<double> d_out, d_work;
-    size_t work_stride = 0, in_bytes = 0, out_doubles = 0;
-    vb::Stream stream;
-    vb::Event ev0, ev1;
-    bool busy = false;
-    std::vector<int> slots;            // members of the launch in flight, by slot
-    std::vector<long long> slot_out;   // their output offsets (doubles)
-    std::chrono::steady_clock::time_point t0;
-    float ms[2] = {0, 0};
-    int launches = 0;
-    vb::LvState* lv = nullptr;  // loop verification (loop_verify.cpp), once enabled
-};
-
-namespace {
 
 // Waits for the batch's launch in flight and copies each member's output block to the member (not yet applied).
 int batch_wait(vp_batch* b) {
@@ -106,7 +45,7 @@ int batch_wait(vp_batch* b) {
     b->ms[0] = ms;
     b->ms[1] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - b->t0).count();
     for (size_t s = 0; s < b->slots.size(); s++) {
-        vp_graph* g = b->members[b->slots[s]];
+        vp_graph* g = b->members[b->slots[s]].get();
         const int n = (int)g->inf_map.size();
         const double* o = b->h_out + b->slot_out[s];
         g->inf_out.assign(o, o + vb::pg_out_layout(n).total);
@@ -122,9 +61,9 @@ int batch_wait(vp_batch* b) {
 int collect(vp_graph* g) {
     if (!g->inflight) return 0;
     if (!g->ready) {
-        const int rc = batch_wait(g->owner);
+        const int rc = batch_wait(g->batch);
         if (rc) {
-            g->err = g->owner->err;
+            g->err = g->batch->err;
             return rc;
         }
     }
@@ -164,46 +103,6 @@ int collect(vp_graph* g) {
     g->last_cost[1] = sm[3];
     g->n_opt++;
     g->inflight = g->ready = false;
-    return 0;
-}
-
-void release(vp_batch* b) {
-    cudaSetDevice(b->cfg.device);
-    vb::lv_release(b->lv);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    for (vp_graph* g : b->members) delete g;
-    delete b;
-}
-
-int batch_create(const vp_config* cfg, int n, vp_batch** out) {
-    *out = nullptr;
-    if (!cfg || n < 1 || cfg->max_keyframes < 2 || cfg->max_anchors < 0 || cfg->max_anchors > vb::PG_CAP_ANCHORS) return VP_ERR_INVALID;
-    if (!vb::device_available(cfg->device)) return VP_ERR_NO_DEVICE;
-    std::unique_ptr<vp_batch, void (*)(vp_batch*)> b(new vp_batch, release);
-    b->cfg = *cfg;
-    b->S = n;
-    b->cap_anchors = cfg->max_anchors ? cfg->max_anchors : vb::PG_MAX_ANCHORS;
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaSetDevice(cfg->device));
-    const int cap = cfg->max_keyframes;
-    b->work_stride = (vb::pg_work_layout(cap, b->cap_anchors).total + 1) & ~(size_t)1;
-    b->in_bytes = vb::pg_arena_bytes(n, cap, b->cap_anchors);
-    b->out_doubles = (size_t)n * vb::pg_out_layout(cap).total;
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->stream.create());
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev0.create());
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev1.create());
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_in.alloc(b->in_bytes));
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_out.alloc(b->out_doubles));
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_in.alloc(b->in_bytes));
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_out.alloc(b->out_doubles));
-    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_work.alloc((size_t)n * b->work_stride));
-    for (int k = 0; k < n; k++) {
-        vp_graph* g = new vp_graph;
-        g->owner = b.get();
-        g->member = k;
-        g->cfg = *cfg;
-        b->members.push_back(g);
-    }
-    *out = b.release();
     return 0;
 }
 
@@ -249,7 +148,7 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, in
     std::sort(anchors.begin(), anchors.end());
     anchors.erase(std::unique(anchors.begin(), anchors.end()), anchors.end());
     const int nb = (int)anchors.size();
-    const int cap = g->owner->cap_anchors;
+    const int cap = g->batch->cap_anchors;
     if (nb > cap) {
         g->err = "vp_optimize: " + std::to_string(nb) + " free loop anchors in the optimised range, at most " + std::to_string(cap);
         return VP_ERR_CAPACITY;
@@ -341,7 +240,7 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
     std::vector<Slot> slots;
     for (int k = 0; k < b->S; k++) {
         if (status) status[k] = 0;
-        vp_graph* g = b->members[k];
+        vp_graph* g = b->members[k].get();
         if ((active && !active[k]) || g->pending < 0) continue;
         int rc = collect(g);  // the member's previous result first
         int n = 0, nb = 0, nc = 0;
@@ -382,7 +281,7 @@ int batch_optimize(vp_batch* b, const int* active, int* status) {
     b->slots.clear();
     b->slot_out.clear();
     for (Slot& sl : slots) {
-        vp_graph* g = b->members[sl.k];
+        vp_graph* g = b->members[sl.k].get();
         b->slots.push_back(sl.k);
         b->slot_out.push_back(sl.out_off);
         g->inflight = true;
@@ -409,38 +308,13 @@ void store_pose(const KeyFrame& kf, double* P3, double* Q4) {
 
 }  // namespace
 
-namespace vb {
-LvState** pg_loop_state(vp_batch* b) { return &b->lv; }
-vp_batch* pg_owner(vp_graph* g, int* member, bool* standalone) {
-    *member = g->member;
-    *standalone = g->standalone;
-    return g->owner;
-}
-int pg_capacity(const vp_batch* b, int* device) {
-    *device = b->cfg.device;
-    return b->cfg.max_keyframes;
-}
-std::string* pg_error(vp_graph* g) { return &g->err; }
-std::string* pg_batch_error(vp_batch* b) { return &b->err; }
-}  // namespace vb
-
 extern "C" {
 
-int vp_create(const vp_config* cfg, vp_graph** out) {
-    if (!out) return VP_ERR_INVALID;
-    vp_batch* b = nullptr;
-    const int rc = batch_create(cfg, 1, &b);
-    if (rc) return rc;
-    b->members[0]->standalone = true;
-    *out = b->members[0];
-    return 0;
-}
+int vp_create(const vp_config* cfg, vp_graph** out) { return vb::create_standalone(vp_batch_create, cfg, out, VP_ERR_INVALID); }
 
-void vp_destroy(vp_graph* g) {
-    if (g && g->standalone) release(g->owner);
-}
+void vp_destroy(vp_graph* g) { vb::destroy_standalone(g, vp_batch_destroy); }
 
-const char* vp_last_error(const vp_graph* g) { return g ? g->err.c_str() : "null handle"; }
+const char* vp_last_error(const vp_graph* g) { return vb::last_error(g); }
 
 int vp_new_sequence(vp_graph* g) {
     if (!g) return VP_ERR_INVALID;
@@ -534,10 +408,10 @@ int vp_update_loop(vp_graph* g, int index, const double* loop_info8) {
 
 int vp_optimize(vp_graph* g) {
     if (!g) return VP_ERR_INVALID;
-    std::vector<int> active(g->owner->S, 0), status(g->owner->S, 0);
+    std::vector<int> active(g->batch->S, 0), status(g->batch->S, 0);
     active[g->member] = 1;
-    const int rc = batch_optimize(g->owner, active.data(), status.data());
-    if (rc && g->err.empty()) g->err = g->owner->err;
+    const int rc = batch_optimize(g->batch, active.data(), status.data());
+    if (rc && g->err.empty()) g->err = g->batch->err;
     return rc ? rc : status[g->member];
 }
 
@@ -639,7 +513,7 @@ int vp_save(vp_graph* g, const char* prefix) {
         m.loop_index = kf.has_loop ? kf.loop_index : -1;
         std::memcpy(m.loop_info, kf.loop_info, sizeof(m.loop_info));
     }
-    vb::LvState* lv = *vb::pg_loop_state(g->owner);
+    vb::LvState* lv = g->batch->lv;
     if (lv) {
         const int r = vb::lv_read_points(lv, g->member, &mk, &g->err);
         if (r) return r;
@@ -654,7 +528,7 @@ int vp_load(vp_graph* g, const char* prefix) {
         g->err = "vp_load: the graph already holds key frames; a map is loaded before the first key frame";
         return VP_ERR_INVALID;
     }
-    vb::LvState* lv = *vb::pg_loop_state(g->owner);
+    vb::LvState* lv = g->batch->lv;
     std::vector<vb::MapKeyFrame> mk;
     int rc = vb::map_read(prefix, lv != nullptr, g->cfg.max_keyframes, lv ? vb::lv_max_corners(lv) : 0, &mk, &g->err);
     if (rc) return rc;
@@ -694,19 +568,50 @@ int vp_load(vp_graph* g, const char* prefix) {
 
 int vp_batch_create(const vp_config* cfg, int n, vp_batch** out) {
     if (!out) return VP_ERR_INVALID;
-    return batch_create(cfg, n, out);
+    *out = nullptr;
+    if (!cfg || n < 1 || cfg->max_keyframes < 2 || cfg->max_anchors < 0 || cfg->max_anchors > vb::PG_CAP_ANCHORS) return VP_ERR_INVALID;
+    if (!vb::device_available(cfg->device)) return VP_ERR_NO_DEVICE;
+    std::unique_ptr<vp_batch, void (*)(vp_batch*)> b(new vp_batch, vp_batch_destroy);
+    b->cfg = *cfg;
+    b->S = n;
+    b->cap_anchors = cfg->max_anchors ? cfg->max_anchors : vb::PG_MAX_ANCHORS;
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, cudaSetDevice(cfg->device));
+    const int cap = cfg->max_keyframes;
+    b->work_stride = (vb::pg_work_layout(cap, b->cap_anchors).total + 1) & ~(size_t)1;
+    b->in_bytes = vb::pg_arena_bytes(n, cap, b->cap_anchors);
+    b->out_doubles = (size_t)n * vb::pg_out_layout(cap).total;
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->stream.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev0.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->ev1.create());
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_in.alloc(b->in_bytes));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->h_out.alloc(b->out_doubles));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_in.alloc(b->in_bytes));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_out.alloc(b->out_doubles));
+    VB_CUDA_CHECK(b, VP_ERR_CUDA, b->d_work.alloc((size_t)n * b->work_stride));
+    for (int k = 0; k < n; k++) {
+        std::unique_ptr<vp_graph> g(new vp_graph);
+        g->batch = b.get();
+        g->member = k;
+        g->cfg = *cfg;
+        b->members.push_back(std::move(g));
+    }
+    *out = b.release();
+    return 0;
 }
 void vp_batch_destroy(vp_batch* b) {
-    if (b) release(b);
+    vb::destroy_batch(b, [b] {
+        vb::lv_release(b->lv);
+        if (b->stream) cudaStreamSynchronize(b->stream);
+    });
 }
-int vp_batch_size(const vp_batch* b) { return b ? b->S : VP_ERR_INVALID; }
-vp_graph* vp_batch_member(vp_batch* b, int k) { return (b && k >= 0 && k < b->S) ? b->members[k] : nullptr; }
-const char* vp_batch_last_error(const vp_batch* b) { return b ? b->err.c_str() : "null handle"; }
+int vp_batch_size(const vp_batch* b) { return vb::batch_size(b, VP_ERR_INVALID); }
+vp_graph* vp_batch_member(vp_batch* b, int k) { return vb::batch_member(b, k); }
+const char* vp_batch_last_error(const vp_batch* b) { return vb::batch_last_error(b); }
 int vp_batch_optimize(vp_batch* b, const int* active, int* status) { return b ? batch_optimize(b, active, status) : VP_ERR_INVALID; }
 int vp_batch_sync(vp_batch* b) {
     if (!b) return VP_ERR_INVALID;
-    for (vp_graph* g : b->members) {
-        const int rc = collect(g);
+    for (auto& g : b->members) {
+        const int rc = collect(g.get());
         if (rc) return rc;
     }
     return 0;

@@ -14,20 +14,16 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <atomic>
 #include <chrono>
 #include <cmath>
-#include <condition_variable>
 #include <cstdio>
 #include <cstring>
-#include <functional>
 #include <map>
 #include <memory>
-#include <mutex>
 #include <string>
-#include <thread>
 #include <vector>
 
+#include "batch_host.h"
 #include "fe_kernels.h"
 #include "fm_ransac.h"
 #include "hostpool.h"
@@ -92,11 +88,8 @@ ArenaSlots arena_slots(const ArenaLayout& a, uint8_t* up, uint8_t* dn, int k) {
 
 }  // namespace
 
-struct vt_tracker {
+struct vt_tracker : vb::MemberBase<vt_batch> {
     vt_config cfg{};
-    std::string err;
-    vt_batch* batch = nullptr;
-    int member = 0;
     // device memory of this member
     vb::DeviceArray<uint8_t> d_lut;
     DevicePyramid pyr[2];
@@ -134,12 +127,8 @@ struct vt_tracker {
     double host_ms_ransac = 0, host_ms_mask = 0;
 };
 
-struct vt_batch {
+struct vt_batch : vb::BatchBase<vt_tracker> {
     vt_config cfg{};
-    int S = 0;
-    bool standalone = false;
-    std::vector<vt_tracker*> members;
-    std::string err;
     vb::Stream stream;
     vb::Event ev0, ev1;
     vb::PinnedArray<vb::FeSeq> h_seq;
@@ -460,7 +449,7 @@ int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_d
     const auto t0 = now();
     b->last_launches = 0;
     b->pool->run(S, [&](int k) {
-        vt_tracker* t = b->members[k];
+        vt_tracker* t = b->members[k].get();
         vb::FeSeq& q = b->h_seq[k];
         q.track = q.detect = 0;
         q.n_pts = 0;
@@ -495,7 +484,7 @@ int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_d
     VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaStreamSynchronize(b->stream));
     const auto t2 = now();
     b->pool->run(S, [&](int k) {
-        if (b->members[k]->step_active) step_after_track(b->members[k]);
+        if (b->members[k]->step_active) step_after_track(b->members[k].get());
     });
     const auto t3 = now();
     for (int k = 0; k < S; k++) {
@@ -519,18 +508,12 @@ int batch_read_image(vt_batch* b, const ImageMsg* msgs, size_t stride, bool on_d
     VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaEventElapsedTime(&b->last_ms, b->ev0, b->ev1));
     const auto t4 = now();
     b->pool->run(S, [&](int k) {
-        if (b->members[k]->step_active) step_finish(b->members[k]);
+        if (b->members[k]->step_active) step_finish(b->members[k].get());
     });
     if (trace)
         std::fprintf(stderr, "[vt_batch] prepare %.3f track(gpu) %.3f host %.3f detect(gpu) %.3f finish %.3f ms (S=%d detect=%d)\n", ms(t0, t1), ms(t1, t2),
                      ms(t2, t3), ms(t3, t4), ms(t4, now()), S, sh.any_detect);
-    int rc = VT_OK;
-    for (int k = 0; k < S; k++)
-        if (b->members[k]->status != VT_OK && rc == VT_OK) {
-            rc = b->members[k]->status;
-            b->err = "member " + std::to_string(k) + ": " + b->members[k]->err;
-        }
-    return rc;
+    return vb::roll_up(b, VT_OK);
 }
 
 // img_callback's gating (feature_tracker_node.cpp:28-62): returns -1 when readImage is due (pub decided), else the
@@ -611,7 +594,7 @@ int create_member(vt_batch* b, int k) {
     t->d = arena_slots(b->ar, b->d_up, b->d_dn, k);
     t->cfg.freq = b->cfg.freq;
     t->cfg.focal_length = b->cfg.focal_length;
-    b->members.push_back(t.release());
+    b->members.push_back(std::move(t));
     return VT_OK;
 }
 
@@ -663,17 +646,15 @@ int vt_batch_create(const vt_config* cfg, int n, vt_batch** out) {
 }
 
 void vt_batch_destroy(vt_batch* b) {
-    if (!b) return;
-    cudaSetDevice(b->cfg.device);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    b->pool.reset();
-    for (auto* t : b->members) delete t;
-    delete b;
+    vb::destroy_batch(b, [b] {
+        if (b->stream) cudaStreamSynchronize(b->stream);
+        b->pool.reset();
+    });
 }
 
-int vt_batch_size(const vt_batch* b) { return b ? b->S : VT_ERR_INVALID; }
-vt_tracker* vt_batch_member(vt_batch* b, int k) { return (b && k >= 0 && k < b->S) ? b->members[k] : nullptr; }
-const char* vt_batch_last_error(const vt_batch* b) { return b ? b->err.c_str() : "null batch"; }
+int vt_batch_size(const vt_batch* b) { return vb::batch_size(b, VT_ERR_INVALID); }
+vt_tracker* vt_batch_member(vt_batch* b, int k) { return vb::batch_member(b, k); }
+const char* vt_batch_last_error(const vt_batch* b) { return vb::batch_last_error(b); }
 
 int vt_batch_read_image(vt_batch* b, const int* active, const uint8_t* const* imgs, size_t row_stride, const double* cur_times,
                         const int* pub_this_frame, int images_on_device) {
@@ -697,7 +678,7 @@ int vt_batch_node_image(vt_batch* b, const int* active, const uint8_t* const* im
         if (active && !active[k]) continue;
         if (!imgs[k]) return VT_ERR_INVALID;
         bool pub = false;
-        const int r = node_gate(b->members[k], stamps[k], restarts ? restarts + k : nullptr, &pub);
+        const int r = node_gate(b->members[k].get(), stamps[k], restarts ? restarts + k : nullptr, &pub);
         if (r >= 0) continue;  // first frame or restart: the image is consumed without tracking
         msgs[k].active = 1;
         msgs[k].pub = pub ? 1 : 0;
@@ -705,7 +686,7 @@ int vt_batch_node_image(vt_batch* b, const int* active, const uint8_t* const* im
     const int rc = batch_read_image(b, msgs.data(), row_stride, images_on_device != 0);
     if (rc) return rc;
     for (int k = 0; k < b->S; k++)
-        if (msgs[k].active) results[k] = node_after(b->members[k], msgs[k].pub != 0);
+        if (msgs[k].active) results[k] = node_after(b->members[k].get(), msgs[k].pub != 0);
     return VT_OK;
 }
 
@@ -716,48 +697,20 @@ int vt_batch_last_timing(const vt_batch* b, float* device_ms, int* kernel_launch
     return VT_OK;
 }
 
-int vt_batch_set_profile(vt_batch* b, int on) {
-    if (!b) return VT_ERR_INVALID;
-    VB_CUDA_CHECK(b, VT_ERR_CUDA, cudaSetDevice(b->cfg.device));
-    b->prof.enable(on != 0);
-    return VT_OK;
-}
+int vt_batch_set_profile(vt_batch* b, int on) { return vb::set_profile(b, on, VT_ERR_INVALID, VT_ERR_CUDA); }
 
-int vt_batch_kernel_times(const vt_batch* b, double* ms6, int* count6) {
-    if (!b) return VT_ERR_INVALID;
-    for (int k = 0; k < 6; k++) {
-        if (ms6) ms6[k] = b->prof.ms[k];
-        if (count6) count6[k] = b->prof.count[k];
-    }
-    return VT_OK;
-}
+int vt_batch_kernel_times(const vt_batch* b, double* ms6, int* count6) { return vb::kernel_times(b, ms6, count6, 6, VT_ERR_INVALID); }
 
-int vt_create(const vt_config* cfg, vt_tracker** out) {
-    if (!cfg || !out) return VT_ERR_INVALID;
-    *out = nullptr;
-    vt_batch* b = nullptr;
-    const int rc = vt_batch_create(cfg, 1, &b);
-    if (rc) return rc;
-    b->standalone = true;
-    *out = b->members[0];
-    return VT_OK;
-}
+int vt_create(const vt_config* cfg, vt_tracker** out) { return vb::create_standalone(vt_batch_create, cfg, out, VT_ERR_INVALID); }
 
-void vt_destroy(vt_tracker* t) {
-    if (t && t->batch && t->batch->standalone) vt_batch_destroy(t->batch);  // members of an explicit batch die with it
-}
+void vt_destroy(vt_tracker* t) { vb::destroy_standalone(t, vt_batch_destroy); }
 
-const char* vt_last_error(const vt_tracker* t) {
-    if (!t) return "null handle";
-    return t->err.empty() && t->batch ? t->batch->err.c_str() : t->err.c_str();
-}
+const char* vt_last_error(const vt_tracker* t) { return vb::last_error(t); }
 
 static int read_image_single(vt_tracker* t, const uint8_t* img, size_t stride, double cur_time, int pub, bool on_device) {
     if (!t || !img || stride < (size_t)t->cfg.cols) return VT_ERR_INVALID;
-    if (!t->batch->standalone) {
-        t->err = "per-handle image call on a member of a batch: use vt_batch_read_image / vt_batch_node_image";
-        return VT_ERR_INVALID;
-    }
+    if (const int rc = vb::refuse_member(t, VT_ERR_INVALID, "per-handle image call on a member of a batch: use vt_batch_read_image / vt_batch_node_image"))
+        return rc;
     t->err.clear();
     ImageMsg m{1, img, cur_time, pub};
     return batch_read_image(t->batch, &m, stride, on_device);
