@@ -218,7 +218,7 @@ __device__ __forceinline__ void prior_dx(const BaProblem& p, const BaStates& x, 
         if (type == 0 || type == 2) {
             const double* xv = type == 0 ? x.pose + 7 * idx : x.ex;
             for (int q = 0; q < 3; q++) dx[off + q] = xv[q] - x0[q];
-            const Q4 dq = qmul(qinv(q_from_param(x0)), q_from_param(xv));
+            const Quat dq = qmul(qinv(q_from_param(x0)), q_from_param(xv));
             const double sg = (dq.w >= 0) ? 2.0 : -2.0;
             dx[off + 3] = sg * dq.x;
             dx[off + 4] = sg * dq.y;

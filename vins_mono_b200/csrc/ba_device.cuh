@@ -1,4 +1,4 @@
-// Device math and residual/Jacobian evaluation of the VINS factors (float64).
+// Residual/Jacobian evaluation of the VINS factors on the device (float64); the rotation arithmetic is rotation.h's.
 //   ProjectionFactor::Evaluate      vins_estimator/src/factor/projection_factor.cpp:21-121
 //   ProjectionTdFactor::Evaluate    vins_estimator/src/factor/projection_td_factor.cpp:34-141
 //   IMUFactor::Evaluate             vins_estimator/src/factor/imu_factor.h:19-179
@@ -9,98 +9,18 @@
 // reference's 2x7 / 15x7 blocks is identically zero and ComputeJacobian is [I6; 0]).
 #pragma once
 #include "ba_types.h"
+#include "rotation.h"
 
 namespace vb {
 
-struct Q4 {
-    double w, x, y, z;
-};
-struct V3d {
-    double x, y, z;
-};
-struct M3d {
-    double m[9];
-};
-
-__device__ __forceinline__ V3d mk(double x, double y, double z) { return V3d{x, y, z}; }
-__device__ __forceinline__ V3d operator+(V3d a, V3d b) { return V3d{a.x + b.x, a.y + b.y, a.z + b.z}; }
-__device__ __forceinline__ V3d operator-(V3d a, V3d b) { return V3d{a.x - b.x, a.y - b.y, a.z - b.z}; }
-__device__ __forceinline__ V3d operator*(V3d a, double s) { return V3d{a.x * s, a.y * s, a.z * s}; }
-__device__ __forceinline__ V3d operator*(double s, V3d a) { return V3d{a.x * s, a.y * s, a.z * s}; }
-__device__ __forceinline__ V3d neg(V3d a) { return V3d{-a.x, -a.y, -a.z}; }
-__device__ __forceinline__ double dot(V3d a, V3d b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ V3d cross(V3d a, V3d b) { return V3d{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
-__device__ __forceinline__ double comp(V3d a, int i) { return i == 0 ? a.x : i == 1 ? a.y : a.z; }
-
-__device__ __forceinline__ Q4 qmul(Q4 a, Q4 b) {
-    return Q4{a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-              a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z, a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x};
-}
-__device__ __forceinline__ Q4 qinv(Q4 q) {
-    const double n2 = q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z;
-    return Q4{q.w / n2, -q.x / n2, -q.y / n2, -q.z / n2};
-}
-__device__ __forceinline__ Q4 qnormalized(Q4 q) {
-    const double n = sqrt(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
-    return Q4{q.w / n, q.x / n, q.y / n, q.z / n};
-}
-__device__ __forceinline__ V3d qrot(Q4 q, V3d v) {  // Eigen's quaternion * vector
-    const V3d u = mk(q.x, q.y, q.z);
-    V3d uv = cross(u, v);
-    uv = uv + uv;
-    return v + q.w * uv + cross(u, uv);
-}
-__device__ __forceinline__ M3d qR(Q4 q) {
-    M3d r;
-    const double tx = 2 * q.x, ty = 2 * q.y, tz = 2 * q.z;
-    const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w;
-    const double txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
-    const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
-    r.m[0] = 1 - (tyy + tzz); r.m[1] = txy - twz;       r.m[2] = txz + twy;
-    r.m[3] = txy + twz;       r.m[4] = 1 - (txx + tzz); r.m[5] = tyz - twx;
-    r.m[6] = txz - twy;       r.m[7] = tyz + twx;       r.m[8] = 1 - (txx + tyy);
-    return r;
-}
-__device__ __forceinline__ Q4 q_from_param(const double* p) { return Q4{p[6], p[3], p[4], p[5]}; }
-__device__ __forceinline__ Q4 deltaQ(V3d th) { return Q4{1.0, th.x / 2.0, th.y / 2.0, th.z / 2.0}; }
-
-__device__ __forceinline__ M3d mmul(const M3d& a, const M3d& b) {
-    M3d r;
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int j = 0; j < 3; j++) r.m[3 * i + j] = a.m[3 * i] * b.m[j] + a.m[3 * i + 1] * b.m[3 + j] + a.m[3 * i + 2] * b.m[6 + j];
-    return r;
-}
-__device__ __forceinline__ M3d mT(const M3d& a) {
-    M3d r;
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int j = 0; j < 3; j++) r.m[3 * i + j] = a.m[3 * j + i];
-    return r;
-}
-__device__ __forceinline__ V3d mv(const M3d& a, V3d v) {
-    return V3d{a.m[0] * v.x + a.m[1] * v.y + a.m[2] * v.z, a.m[3] * v.x + a.m[4] * v.y + a.m[5] * v.z, a.m[6] * v.x + a.m[7] * v.y + a.m[8] * v.z};
-}
-__device__ __forceinline__ M3d skew(V3d q) {
-    M3d r;
-    r.m[0] = 0;    r.m[1] = -q.z; r.m[2] = q.y;
-    r.m[3] = q.z;  r.m[4] = 0;    r.m[5] = -q.x;
-    r.m[6] = -q.y; r.m[7] = q.x;  r.m[8] = 0;
-    return r;
-}
-__device__ __forceinline__ M3d mscale(const M3d& a, double s) { M3d r; for (int i = 0; i < 9; i++) r.m[i] = a.m[i] * s; return r; }
-__device__ __forceinline__ M3d madd(const M3d& a, const M3d& b) { M3d r; for (int i = 0; i < 9; i++) r.m[i] = a.m[i] + b.m[i]; return r; }
-__device__ __forceinline__ M3d msub(const M3d& a, const M3d& b) { M3d r; for (int i = 0; i < 9; i++) r.m[i] = a.m[i] - b.m[i]; return r; }
-__device__ __forceinline__ M3d mident() { M3d r; for (int i = 0; i < 9; i++) r.m[i] = (i % 4 == 0) ? 1.0 : 0.0; return r; }
+__device__ __forceinline__ Quat q_from_param(const double* p) { return Quat{p[6], p[3], p[4], p[5]}; }
 
 // PoseLocalParameterization::Plus
 __device__ __forceinline__ void pose_plus(const double* x, const double* d, double* out) {
     out[0] = x[0] + d[0];
     out[1] = x[1] + d[1];
     out[2] = x[2] + d[2];
-    const Q4 q = qnormalized(qmul(q_from_param(x), deltaQ(mk(d[3], d[4], d[5]))));
+    const Quat q = qnormalized(qmul(q_from_param(x), deltaQ(Vec3(d[3], d[4], d[5]))));
     out[3] = q.x;
     out[4] = q.y;
     out[5] = q.z;
@@ -144,20 +64,20 @@ __device__ __forceinline__ void eval_visual(const BaDims& d, const double* pose_
                                             double inv_dep_i, double td, double pix, double piy, double pjx, double pjy,
                                             double vix, double viy, double vjx, double vjy, double td_i, double td_j,
                                             double row_i, double row_j, bool want_jac, bool robust, VisualEval& e) {
-    V3d pts_i = mk(pix, piy, 1.0), pts_j = mk(pjx, pjy, 1.0);
+    Vec3 pts_i = Vec3(pix, piy, 1.0), pts_j = Vec3(pjx, pjy, 1.0);
     if (d.est_td) {  // ProjectionTdFactor
         const double ci = td - td_i + d.tr_over_row * (row_i - d.half_row);
         const double cj = td - td_j + d.tr_over_row * (row_j - d.half_row);
-        pts_i = pts_i - ci * mk(vix, viy, 0.0);
-        pts_j = pts_j - cj * mk(vjx, vjy, 0.0);
+        pts_i = pts_i - ci * Vec3(vix, viy, 0.0);
+        pts_j = pts_j - cj * Vec3(vjx, vjy, 0.0);
     }
-    const V3d Pi = mk(pose_i[0], pose_i[1], pose_i[2]), Pj = mk(pose_j[0], pose_j[1], pose_j[2]), tic = mk(ex[0], ex[1], ex[2]);
-    const Q4 Qi = q_from_param(pose_i), Qj = q_from_param(pose_j), qic = q_from_param(ex);
-    const V3d pci = mk(pts_i.x / inv_dep_i, pts_i.y / inv_dep_i, pts_i.z / inv_dep_i);
-    const V3d pts_imu_i = qrot(qic, pci) + tic;
-    const V3d pts_w = qrot(Qi, pts_imu_i) + Pi;
-    const V3d pts_imu_j = qrot(qinv(Qj), pts_w - Pj);
-    const V3d pcj = qrot(qinv(qic), pts_imu_j - tic);
+    const Vec3 Pi = Vec3(pose_i[0], pose_i[1], pose_i[2]), Pj = Vec3(pose_j[0], pose_j[1], pose_j[2]), tic = Vec3(ex[0], ex[1], ex[2]);
+    const Quat Qi = q_from_param(pose_i), Qj = q_from_param(pose_j), qic = q_from_param(ex);
+    const Vec3 pci = Vec3(pts_i.x / inv_dep_i, pts_i.y / inv_dep_i, pts_i.z / inv_dep_i);
+    const Vec3 pts_imu_i = qrot(qic, pci) + tic;
+    const Vec3 pts_w = qrot(Qi, pts_imu_i) + Pi;
+    const Vec3 pts_imu_j = qrot(qinv(Qj), pts_w - Pj);
+    const Vec3 pcj = qrot(qinv(qic), pts_imu_j - tic);
     const double dep_j = pcj.z;
     const double s = d.sqrt_info_vis;
     e.r[0] = s * (pcj.x / dep_j - pts_j.x);
@@ -167,23 +87,23 @@ __device__ __forceinline__ void eval_visual(const BaDims& d, const double* pose_
     if (robust) c = cauchy_corrector(sq);
     e.half_rho = c.half_rho0;
     if (want_jac) {
-        const M3d Ri = qR(Qi), Rj = qR(Qj), ric = qR(qic);
-        const M3d ricT = mT(ric), RjT = mT(Rj);
+        const Mat3 Ri = qR(Qi), Rj = qR(Qj), ric = qR(qic);
+        const Mat3 ricT = mT(ric), RjT = mT(Rj);
         double red[2][3];
         red[0][0] = s * (1. / dep_j); red[0][1] = 0; red[0][2] = s * (-pcj.x / (dep_j * dep_j));
         red[1][0] = 0; red[1][1] = s * (1. / dep_j); red[1][2] = s * (-pcj.y / (dep_j * dep_j));
-        const M3d A = mmul(ricT, RjT);                       // d pcj / d Pi
-        const M3d B = mmul(mmul(A, Ri), mscale(skew(pts_imu_i), -1.0));
-        const M3d Cm = mscale(A, -1.0);                      // d pcj / d Pj
-        const M3d Dm = mmul(ricT, skew(pts_imu_j));
-        const M3d tmp_r = mmul(mmul(A, Ri), ric);
-        M3d Eex, Fex;
+        const Mat3 A = mmul(ricT, RjT);                       // d pcj / d Pi
+        const Mat3 B = mmul(mmul(A, Ri), mscale(skew(pts_imu_i), -1.0));
+        const Mat3 Cm = mscale(A, -1.0);                      // d pcj / d Pj
+        const Mat3 Dm = mmul(ricT, skew(pts_imu_j));
+        const Mat3 tmp_r = mmul(mmul(A, Ri), ric);
+        Mat3 Eex, Fex;
         if (EX) {
-            Eex = mmul(ricT, msub(mmul(RjT, Ri), mident()));
-            const V3d inner = mv(RjT, mv(Ri, tic) + Pi - Pj) - tic;
+            Eex = mmul(ricT, msub(mmul(RjT, Ri), Mat3()));
+            const Vec3 inner = mv(RjT, mv(Ri, tic) + Pi - Pj) - tic;
             Fex = madd(madd(mscale(mmul(tmp_r, skew(pci)), -1.0), skew(mv(tmp_r, pci))), skew(mv(ricT, inner)));
         }
-        const V3d dl = mv(tmp_r, pts_i) * (-1.0 / (inv_dep_i * inv_dep_i));
+        const Vec3 dl = mv(tmp_r, pts_i) * (-1.0 / (inv_dep_i * inv_dep_i));
 #pragma unroll
         for (int rr = 0; rr < 2; rr++) {
 #pragma unroll
@@ -204,8 +124,8 @@ __device__ __forceinline__ void eval_visual(const BaDims& d, const double* pose_
             e.J[rr][19] = 0.0;
         }
         if (TD && d.est_td) {
-            const V3d vi = mk(vix, viy, 0.0);
-            const V3d dtd = mv(tmp_r, vi) * (-1.0 / inv_dep_i);
+            const Vec3 vi = Vec3(vix, viy, 0.0);
+            const Vec3 dtd = mv(tmp_r, vi) * (-1.0 / inv_dep_i);
             e.J[0][19] = red[0][0] * dtd.x + red[0][1] * dtd.y + red[0][2] * dtd.z + s * vjx;
             e.J[1][19] = red[1][0] * dtd.x + red[1][1] * dtd.y + red[1][2] * dtd.z + s * vjy;
         }
@@ -225,18 +145,18 @@ __device__ __forceinline__ void eval_visual(const BaDims& d, const double* pose_
 }
 
 // bottom-right 3x3 of Qleft(a) and of Qleft(a) * Qright(b)  (utility.h:51-68)
-__device__ __forceinline__ M3d qleft_br(Q4 q) { return madd(mscale(mident(), q.w), skew(mk(q.x, q.y, q.z))); }
-__device__ __forceinline__ M3d qleft_qright_br(Q4 a, Q4 b) {
+__device__ __forceinline__ Mat3 qleft_br(Quat q) { return madd(mscale(Mat3(), q.w), skew(Vec3(q.x, q.y, q.z))); }
+__device__ __forceinline__ Mat3 qleft_qright_br(Quat a, Quat b) {
     // rows 1..3 of Qleft(a) times columns 1..3 of Qright(b)
-    const V3d av = mk(a.x, a.y, a.z), bv = mk(b.x, b.y, b.z);
-    const M3d La = madd(mscale(mident(), a.w), skew(av));
-    const M3d Rb = msub(mscale(mident(), b.w), skew(bv));
-    M3d r = mmul(La, Rb);
+    const Vec3 av = Vec3(a.x, a.y, a.z), bv = Vec3(b.x, b.y, b.z);
+    const Mat3 La = madd(mscale(Mat3(), a.w), skew(av));
+    const Mat3 Rb = msub(mscale(Mat3(), b.w), skew(bv));
+    Mat3 r = mmul(La, Rb);
     // + a.vec * (-b.vec)^T  (column 0 of Qleft rows 1..3 times row 0 of Qright cols 1..3)
 #pragma unroll
     for (int i = 0; i < 3; i++)
 #pragma unroll
-        for (int j = 0; j < 3; j++) r.m[3 * i + j] += comp(av, i) * (-comp(bv, j));
+        for (int j = 0; j < 3; j++) r.m[3 * i + j] += av[i] * (-bv[j]);
     return r;
 }
 
@@ -244,50 +164,50 @@ __device__ __forceinline__ M3d qleft_qright_br(Q4 a, Q4 b) {
 // [pose_i(6) | speedbias_i(9) | pose_j(6) | speedbias_j(9)] (row-major, zero-initialised by the caller).
 __device__ inline void eval_imu_raw(const BaDims& d, const PreInt& pre, const double* pose_i, const double* sb_i,
                                     const double* pose_j, const double* sb_j, double* r, double* Jraw /* may be null */) {
-    const V3d Pi = mk(pose_i[0], pose_i[1], pose_i[2]), Pj = mk(pose_j[0], pose_j[1], pose_j[2]);
-    const Q4 Qi = q_from_param(pose_i), Qj = q_from_param(pose_j);
-    const V3d Vi = mk(sb_i[0], sb_i[1], sb_i[2]), Bai = mk(sb_i[3], sb_i[4], sb_i[5]), Bgi = mk(sb_i[6], sb_i[7], sb_i[8]);
-    const V3d Vj = mk(sb_j[0], sb_j[1], sb_j[2]), Baj = mk(sb_j[3], sb_j[4], sb_j[5]), Bgj = mk(sb_j[6], sb_j[7], sb_j[8]);
-    const V3d G = mk(d.G[0], d.G[1], d.G[2]);
+    const Vec3 Pi = Vec3(pose_i[0], pose_i[1], pose_i[2]), Pj = Vec3(pose_j[0], pose_j[1], pose_j[2]);
+    const Quat Qi = q_from_param(pose_i), Qj = q_from_param(pose_j);
+    const Vec3 Vi = Vec3(sb_i[0], sb_i[1], sb_i[2]), Bai = Vec3(sb_i[3], sb_i[4], sb_i[5]), Bgi = Vec3(sb_i[6], sb_i[7], sb_i[8]);
+    const Vec3 Vj = Vec3(sb_j[0], sb_j[1], sb_j[2]), Baj = Vec3(sb_j[3], sb_j[4], sb_j[5]), Bgj = Vec3(sb_j[6], sb_j[7], sb_j[8]);
+    const Vec3 G = Vec3(d.G[0], d.G[1], d.G[2]);
     const double sum_dt = pre.sum_dt;
     auto blk = [&](int r0, int c0) {
-        M3d b;
+        Mat3 b;
 #pragma unroll
         for (int i = 0; i < 3; i++)
 #pragma unroll
             for (int j = 0; j < 3; j++) b.m[3 * i + j] = pre.jac[(r0 + i) * 15 + c0 + j];
         return b;
     };
-    const M3d dp_dba = blk(0, 9), dp_dbg = blk(0, 12), dq_dbg = blk(3, 12), dv_dba = blk(6, 9), dv_dbg = blk(6, 12);
-    const V3d dba = Bai - mk(pre.ba[0], pre.ba[1], pre.ba[2]), dbg = Bgi - mk(pre.bg[0], pre.bg[1], pre.bg[2]);
-    const Q4 delta_q = Q4{pre.dq[0], pre.dq[1], pre.dq[2], pre.dq[3]};
-    const Q4 corrected_delta_q = qmul(delta_q, deltaQ(mv(dq_dbg, dbg)));
-    const V3d corrected_delta_v = mk(pre.dv[0], pre.dv[1], pre.dv[2]) + mv(dv_dba, dba) + mv(dv_dbg, dbg);
-    const V3d corrected_delta_p = mk(pre.dp[0], pre.dp[1], pre.dp[2]) + mv(dp_dba, dba) + mv(dp_dbg, dbg);
-    const Q4 Qi_inv = qinv(Qi);
-    const V3d tp = qrot(Qi_inv, 0.5 * G * sum_dt * sum_dt + Pj - Pi - Vi * sum_dt);
-    const V3d tv = qrot(Qi_inv, G * sum_dt + Vj - Vi);
-    const V3d rp = tp - corrected_delta_p;
-    const Q4 qe = qmul(qinv(corrected_delta_q), qmul(Qi_inv, Qj));
-    const V3d rq = 2.0 * mk(qe.x, qe.y, qe.z);
-    const V3d rv = tv - corrected_delta_v;
-    const V3d rba = Baj - Bai, rbg = Bgj - Bgi;
+    const Mat3 dp_dba = blk(0, 9), dp_dbg = blk(0, 12), dq_dbg = blk(3, 12), dv_dba = blk(6, 9), dv_dbg = blk(6, 12);
+    const Vec3 dba = Bai - Vec3(pre.ba[0], pre.ba[1], pre.ba[2]), dbg = Bgi - Vec3(pre.bg[0], pre.bg[1], pre.bg[2]);
+    const Quat delta_q = Quat{pre.dq[0], pre.dq[1], pre.dq[2], pre.dq[3]};
+    const Quat corrected_delta_q = qmul(delta_q, deltaQ(mv(dq_dbg, dbg)));
+    const Vec3 corrected_delta_v = Vec3(pre.dv[0], pre.dv[1], pre.dv[2]) + mv(dv_dba, dba) + mv(dv_dbg, dbg);
+    const Vec3 corrected_delta_p = Vec3(pre.dp[0], pre.dp[1], pre.dp[2]) + mv(dp_dba, dba) + mv(dp_dbg, dbg);
+    const Quat Qi_inv = qinv(Qi);
+    const Vec3 tp = qrot(Qi_inv, 0.5 * G * sum_dt * sum_dt + Pj - Pi - Vi * sum_dt);
+    const Vec3 tv = qrot(Qi_inv, G * sum_dt + Vj - Vi);
+    const Vec3 rp = tp - corrected_delta_p;
+    const Quat qe = qmul(qinv(corrected_delta_q), qmul(Qi_inv, Qj));
+    const Vec3 rq = 2.0 * Vec3(qe.x, qe.y, qe.z);
+    const Vec3 rv = tv - corrected_delta_v;
+    const Vec3 rba = Baj - Bai, rbg = Bgj - Bgi;
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-        r[i] = comp(rp, i);
-        r[3 + i] = comp(rq, i);
-        r[6 + i] = comp(rv, i);
-        r[9 + i] = comp(rba, i);
-        r[12 + i] = comp(rbg, i);
+        r[i] = rp[i];
+        r[3 + i] = rq[i];
+        r[6 + i] = rv[i];
+        r[9 + i] = rba[i];
+        r[12 + i] = rbg[i];
     }
     if (!Jraw) return;
-    auto put = [&](int r0, int c0, const M3d& b) {
+    auto put = [&](int r0, int c0, const Mat3& b) {
 #pragma unroll
         for (int i = 0; i < 3; i++)
 #pragma unroll
             for (int j = 0; j < 3; j++) Jraw[(r0 + i) * 30 + c0 + j] = b.m[3 * i + j];
     };
-    const M3d RiT = qR(Qi_inv), I3 = mident();
+    const Mat3 RiT = qR(Qi_inv), I3 = Mat3();
     // pose_i: cols 0..5
     put(0, 0, mscale(RiT, -1.0));
     put(0, 3, skew(tp));
@@ -310,51 +230,6 @@ __device__ inline void eval_imu_raw(const BaDims& d, const PreInt& pre, const do
     put(6, 21, RiT);
     put(9, 24, I3);
     put(12, 27, I3);
-}
-
-// Utility::R2ypr / ypr2R (utility.h:70-112, degrees) and Eigen's rotation-matrix -> quaternion conversion, used by the
-// device-side double2vector / vector2double.
-__device__ inline V3d R2ypr_dev(const M3d& R) {
-    const V3d n = mk(R.m[0], R.m[3], R.m[6]), o = mk(R.m[1], R.m[4], R.m[7]), a = mk(R.m[2], R.m[5], R.m[8]);
-    const double y = atan2(n.y, n.x);
-    const double p = atan2(-n.z, n.x * cos(y) + n.y * sin(y));
-    const double r = atan2(a.x * sin(y) - a.y * cos(y), -o.x * sin(y) + o.y * cos(y));
-    return mk(y, p, r) * (1.0 / 3.14159265358979323846 * 180.0);
-}
-__device__ inline M3d ypr2R_dev(V3d ypr) {
-    const double y = ypr.x / 180.0 * 3.14159265358979323846, p = ypr.y / 180.0 * 3.14159265358979323846,
-                 r = ypr.z / 180.0 * 3.14159265358979323846;
-    M3d Rz = mident(), Ry = mident(), Rx = mident();
-    Rz.m[0] = cos(y); Rz.m[1] = -sin(y); Rz.m[3] = sin(y); Rz.m[4] = cos(y);
-    Ry.m[0] = cos(p); Ry.m[2] = sin(p); Ry.m[6] = -sin(p); Ry.m[8] = cos(p);
-    Rx.m[4] = cos(r); Rx.m[5] = -sin(r); Rx.m[7] = sin(r); Rx.m[8] = cos(r);
-    return mmul(mmul(Rz, Ry), Rx);
-}
-__device__ inline Q4 q_from_R(const M3d& m) {
-    Q4 q;
-    double t = m.m[0] + m.m[4] + m.m[8];
-    if (t > 0) {
-        t = sqrt(t + 1.0);
-        q.w = 0.5 * t;
-        t = 0.5 / t;
-        q.x = (m.m[7] - m.m[5]) * t;
-        q.y = (m.m[2] - m.m[6]) * t;
-        q.z = (m.m[3] - m.m[1]) * t;
-    } else {
-        int i = 0;
-        if (m.m[4] > m.m[0]) i = 1;
-        if (m.m[8] > m.m[4 * i]) i = 2;
-        const int j = (i + 1) % 3, k = (j + 1) % 3;
-        t = sqrt(m.m[4 * i] - m.m[4 * j] - m.m[4 * k] + 1.0);
-        double c[3];
-        c[i] = 0.5 * t;
-        t = 0.5 / t;
-        q.w = (m.m[3 * k + j] - m.m[3 * j + k]) * t;
-        c[j] = (m.m[3 * j + i] + m.m[3 * i + j]) * t;
-        c[k] = (m.m[3 * k + i] + m.m[3 * i + k]) * t;
-        q.x = c[0]; q.y = c[1]; q.z = c[2];
-    }
-    return q;
 }
 
 __device__ __forceinline__ double warp_sum_d(double v) {

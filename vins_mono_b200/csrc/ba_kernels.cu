@@ -50,31 +50,31 @@ __device__ void preint_push_dev(PreInt* __restrict__ slot, int n, const double* 
         st[16] = slot->sum_dt;
     }
     __syncthreads();
-    const V3d ba = mk(slot->ba[0], slot->ba[1], slot->ba[2]), bg = mk(slot->bg[0], slot->bg[1], slot->bg[2]);
+    const Vec3 ba = Vec3(slot->ba[0], slot->ba[1], slot->ba[2]), bg = Vec3(slot->bg[0], slot->bg[1], slot->bg[2]);
     for (int k = 0; k < n; k++) {
         for (int i = tid; i < 225; i += 256) F[i] = 0.0;
         for (int i = tid; i < 270; i += 256) V[i] = 0.0;
         __syncthreads();
         if (tid == 0) {
             const double dt = samples[7 * k];
-            const V3d a1 = mk(samples[7 * k + 1], samples[7 * k + 2], samples[7 * k + 3]);
-            const V3d g1 = mk(samples[7 * k + 4], samples[7 * k + 5], samples[7 * k + 6]);
-            const V3d a0 = mk(st[10], st[11], st[12]), g0 = mk(st[13], st[14], st[15]);
-            const V3d dp = mk(st[0], st[1], st[2]), dv = mk(st[7], st[8], st[9]);
-            const Q4 dq = Q4{st[3], st[4], st[5], st[6]};
-            const V3d un_acc_0 = qrot(dq, a0 - ba);
-            const V3d un_gyr = 0.5 * (g0 + g1) - bg;
-            const Q4 rq = qmul(dq, Q4{1, un_gyr.x * dt / 2, un_gyr.y * dt / 2, un_gyr.z * dt / 2});
-            const V3d un_acc_1 = qrot(rq, a1 - ba);
-            const V3d un_acc = 0.5 * (un_acc_0 + un_acc_1);
-            const V3d rdp = dp + dv * dt + 0.5 * un_acc * dt * dt;
-            const V3d rdv = dv + un_acc * dt;
-            const M3d Rwx = skew(un_gyr), Ra0 = skew(a0 - ba), Ra1 = skew(a1 - ba);
-            const M3d Rq = qR(dq), Rr = qR(rq), I = mident();
-            const M3d ImW = msub(I, mscale(Rwx, dt));
-            auto putF = [&](int r0, int c0, const M3d& b) { for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) F[(r0 + i) * 15 + c0 + j] = b.m[3 * i + j]; };
-            auto putV = [&](int r0, int c0, const M3d& b) { for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) V[(r0 + i) * 18 + c0 + j] = b.m[3 * i + j]; };
-            const M3d RqA0 = mmul(Rq, Ra0), RrA1 = mmul(Rr, Ra1), RrA1W = mmul(RrA1, ImW);
+            const Vec3 a1 = Vec3(samples[7 * k + 1], samples[7 * k + 2], samples[7 * k + 3]);
+            const Vec3 g1 = Vec3(samples[7 * k + 4], samples[7 * k + 5], samples[7 * k + 6]);
+            const Vec3 a0 = Vec3(st[10], st[11], st[12]), g0 = Vec3(st[13], st[14], st[15]);
+            const Vec3 dp = Vec3(st[0], st[1], st[2]), dv = Vec3(st[7], st[8], st[9]);
+            const Quat dq = Quat{st[3], st[4], st[5], st[6]};
+            const Vec3 un_acc_0 = qrot(dq, a0 - ba);
+            const Vec3 un_gyr = 0.5 * (g0 + g1) - bg;
+            const Quat rq = qmul(dq, Quat{1, un_gyr.x * dt / 2, un_gyr.y * dt / 2, un_gyr.z * dt / 2});
+            const Vec3 un_acc_1 = qrot(rq, a1 - ba);
+            const Vec3 un_acc = 0.5 * (un_acc_0 + un_acc_1);
+            const Vec3 rdp = dp + dv * dt + 0.5 * un_acc * dt * dt;
+            const Vec3 rdv = dv + un_acc * dt;
+            const Mat3 Rwx = skew(un_gyr), Ra0 = skew(a0 - ba), Ra1 = skew(a1 - ba);
+            const Mat3 Rq = qR(dq), Rr = qR(rq), I = Mat3();
+            const Mat3 ImW = msub(I, mscale(Rwx, dt));
+            auto putF = [&](int r0, int c0, const Mat3& b) { for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) F[(r0 + i) * 15 + c0 + j] = b.m[3 * i + j]; };
+            auto putV = [&](int r0, int c0, const Mat3& b) { for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) V[(r0 + i) * 18 + c0 + j] = b.m[3 * i + j]; };
+            const Mat3 RqA0 = mmul(Rq, Ra0), RrA1 = mmul(Rr, Ra1), RrA1W = mmul(RrA1, ImW);
             putF(0, 0, I);
             putF(0, 3, madd(mscale(RqA0, -0.25 * dt * dt), mscale(RrA1W, -0.25 * dt * dt)));
             putF(0, 6, mscale(I, dt));
@@ -88,7 +88,7 @@ __device__ void preint_push_dev(PreInt* __restrict__ slot, int n, const double* 
             putF(6, 12, mscale(RrA1, -0.5 * dt * -dt));
             putF(9, 9, I);
             putF(12, 12, I);
-            const M3d v03 = mscale(RrA1, 0.25 * -1.0 * dt * dt * 0.5 * dt), v63 = mscale(RrA1, 0.5 * -1.0 * dt * 0.5 * dt);
+            const Mat3 v03 = mscale(RrA1, 0.25 * -1.0 * dt * dt * 0.5 * dt), v63 = mscale(RrA1, 0.5 * -1.0 * dt * 0.5 * dt);
             putV(0, 0, mscale(Rq, 0.25 * dt * dt));
             putV(0, 3, v03);
             putV(0, 6, mscale(Rr, 0.25 * dt * dt));
@@ -101,7 +101,7 @@ __device__ void preint_push_dev(PreInt* __restrict__ slot, int n, const double* 
             putV(6, 9, v63);
             putV(9, 12, mscale(I, dt));
             putV(12, 15, mscale(I, dt));
-            const Q4 nq = qnormalized(rq);
+            const Quat nq = qnormalized(rq);
             st[0] = rdp.x; st[1] = rdp.y; st[2] = rdp.z;
             st[3] = nq.w; st[4] = nq.x; st[5] = nq.y; st[6] = nq.z;
             st[7] = rdv.x; st[8] = rdv.y; st[9] = rdv.z;
@@ -1195,13 +1195,13 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
     if (tid == 0) sx.td[0] = xs.td[0];
     __syncthreads();
     if (tid == 0) {
-        const M3d R00 = qR(q_from_param(sx.pose));
-        const V3d o0 = mk(fp.origin_ypr[0], fp.origin_ypr[1], fp.origin_ypr[2]);
-        const V3d o00 = R2ypr_dev(R00);
+        const Mat3 R00 = qR(q_from_param(sx.pose));
+        const Vec3 o0 = Vec3(fp.origin_ypr[0], fp.origin_ypr[1], fp.origin_ypr[2]);
+        const Vec3 o00 = R2ypr(R00);
         const double y_diff = o0.x - o00.x;
-        M3d rd = ypr2R_dev(mk(y_diff, 0.0, 0.0));
+        Mat3 rd = ypr2R(Vec3(y_diff, 0.0, 0.0));
         if (fabs(fabs(o0.y) - 90) < 1.0 || fabs(fabs(o00.y) - 90) < 1.0) {
-            M3d R0;
+            Mat3 R0;
             for (int k = 0; k < 9; k++) R0.m[k] = fp.Rs0[k];
             rd = mmul(R0, mT(R00));
         }
@@ -1214,21 +1214,21 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
         for (int i = tid; i < (int)(sizeof(SolverState) / 8); i += nt) reinterpret_cast<unsigned long long*>(out)[i] = src[i];
     }
     const BaOutLayout ol = ba_out_layout(F, L, p.dims.col_relo >= 0);
-    M3d rd;
+    Mat3 rd;
     for (int k = 0; k < 9; k++) rd.m[k] = rot[k];
     for (int f = tid; f < F; f += nt) {
         const double* pp = sx.pose + 7 * f;
         const double* sbp = sx.sb + 9 * f;
-        const M3d R = mmul(rd, qR(qnormalized(q_from_param(pp))));
-        const V3d P = mv(rd, mk(pp[0] - sx.pose[0], pp[1] - sx.pose[1], pp[2] - sx.pose[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
-        const V3d V = mv(rd, mk(sbp[0], sbp[1], sbp[2]));
+        const Mat3 R = mmul(rd, qR(qnormalized(q_from_param(pp))));
+        const Vec3 P = mv(rd, Vec3(pp[0] - sx.pose[0], pp[1] - sx.pose[1], pp[2] - sx.pose[2])) + Vec3(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
+        const Vec3 V = mv(rd, Vec3(sbp[0], sbp[1], sbp[2]));
         double* o = out + ol.frames + BA_OUT_FRAME * f;
         o[0] = P.x; o[1] = P.y; o[2] = P.z;
         for (int k = 0; k < 9; k++) o[3 + k] = R.m[k];
         o[12] = V.x; o[13] = V.y; o[14] = V.z;
         for (int k = 0; k < 6; k++) o[15 + k] = sbp[3 + k];
         // vector2double
-        const Q4 qq = q_from_R(R);
+        const Quat qq = Quat::FromR(R);
         double* dp = xd.pose + 7 * f;
         dp[0] = P.x; dp[1] = P.y; dp[2] = P.z; dp[3] = qq.x; dp[4] = qq.y; dp[5] = qq.z; dp[6] = qq.w;
         double* ds = xd.sb + 9 * f;
@@ -1237,20 +1237,20 @@ __global__ void __launch_bounds__(128) ba_finish_kernel(BaSeq* __restrict__ seqs
     }
     if (tid == nt - 1) {
         const double* xe = sx.ex;
-        const M3d ric = qR(q_from_param(xe));
+        const Mat3 ric = qR(q_from_param(xe));
         double* o = out + ol.ex;
         o[0] = xe[0]; o[1] = xe[1]; o[2] = xe[2];
         for (int k = 0; k < 9; k++) o[3 + k] = ric.m[k];
         o[12] = sx.td[0];
-        const Q4 qq = q_from_R(ric);
+        const Quat qq = Quat::FromR(ric);
         xd.ex[0] = xe[0]; xd.ex[1] = xe[1]; xd.ex[2] = xe[2];
         xd.ex[3] = qq.x; xd.ex[4] = qq.y; xd.ex[5] = qq.z; xd.ex[6] = qq.w;
         xd.td[0] = sx.td[0];
     }
     if (tid == nt - 2 && p.dims.col_relo >= 0) {  // relo_r / relo_t of double2vector (estimator.cpp:598-605)
         const double* rp = xs.relo;
-        const M3d Rr = mmul(rd, qR(qnormalized(q_from_param(rp))));
-        const V3d Pr = mv(rd, mk(rp[0] - sx.pose[0], rp[1] - sx.pose[1], rp[2] - sx.pose[2])) + mk(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
+        const Mat3 Rr = mmul(rd, qR(qnormalized(q_from_param(rp))));
+        const Vec3 Pr = mv(rd, Vec3(rp[0] - sx.pose[0], rp[1] - sx.pose[1], rp[2] - sx.pose[2])) + Vec3(fp.origin_P0[0], fp.origin_P0[1], fp.origin_P0[2]);
         double* o = out + ol.relo;
         for (int k = 0; k < 9; k++) o[k] = Rr.m[k];
         o[9] = Pr.x; o[10] = Pr.y; o[11] = Pr.z;

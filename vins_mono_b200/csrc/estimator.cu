@@ -27,14 +27,14 @@
 #include "ba_layout.h"
 #include "batch_host.h"
 #include "cuda_check.h"
-#include "host_math.h"
 #include "hostpool.h"
 #include "initial.h"
+#include "rotation.h"
 #include "vinsb200/estimator.h"
 
-using hm::Mat3;
-using hm::Quat;
-using hm::Vec3;
+using vb::Mat3;
+using vb::Quat;
+using vb::Vec3;
 
 namespace {
 
@@ -314,7 +314,7 @@ void triangulate(ve_estimator* e) {
             row += 2;
         }
         double v[4];
-        hm::null_direction4(A, row, v);
+        vb::null_direction4(A, row, v);
         it.estimated_depth = v[2] / v[3];
         if (it.estimated_depth < 0.1) it.estimated_depth = e->cfg.init_depth;
     }
@@ -427,7 +427,7 @@ void process_imu(ve_estimator* e, double dt, const Vec3& acc, const Vec3& gyr) {
         if (e->solver_flag == 0 && e->tmp_pre.valid) e->tmp_pre.push_back(dt, acc, gyr);  // tmp_pre_integration->push_back
         const Vec3 un_acc_0 = e->Rs[j] * (e->acc_0 - e->Bas[j]) - e->g;
         const Vec3 un_gyr = 0.5 * (e->gyr_0 + gyr) - e->Bgs[j];
-        e->Rs[j] = e->Rs[j] * hm::deltaQ_R(un_gyr * dt);
+        e->Rs[j] = e->Rs[j] * vb::deltaQ(un_gyr * dt).R();
         const Vec3 un_acc_1 = e->Rs[j] * (acc - e->Bas[j]) - e->g;
         const Vec3 un_acc = 0.5 * (un_acc_0 + un_acc_1);
         e->Ps[j] += dt * e->Vs[j] + 0.5 * dt * dt * un_acc;
@@ -545,8 +545,8 @@ bool initial_structure(ve_estimator* e) {
         it.estimated_depth *= s;
     }
     Mat3 R0 = vi::g2R(res.g);
-    const double yaw = hm::R2ypr(R0 * e->Rs[0]).x;
-    R0 = hm::ypr2R(Vec3(-yaw, 0, 0)) * R0;
+    const double yaw = vb::R2ypr(R0 * e->Rs[0]).x;
+    R0 = vb::ypr2R(Vec3(-yaw, 0, 0)) * R0;
     e->g = R0 * res.g;
     for (int i = 0; i <= e->frame_count; i++) {
         e->Ps[i] = R0 * e->Ps[i];
@@ -622,16 +622,13 @@ void unpack_results(ve_estimator* e, const double* out) {
         Mat3 relo_r;
         std::memcpy(relo_r.m, ro, 9 * sizeof(double));
         const Vec3 relo_t(ro[9], ro[10], ro[11]);
-        const double drift_correct_yaw = hm::R2ypr(e->prev_relo_r).x - hm::R2ypr(relo_r).x;
-        e->drift_correct_r = hm::ypr2R(Vec3(drift_correct_yaw, 0, 0));
+        const double drift_correct_yaw = vb::R2ypr(e->prev_relo_r).x - vb::R2ypr(relo_r).x;
+        e->drift_correct_r = vb::ypr2R(Vec3(drift_correct_yaw, 0, 0));
         e->drift_correct_t = e->prev_relo_t - e->drift_correct_r * relo_t;
         const int li = e->relo_frame_local_index;
         e->relo_relative_t = relo_r.T() * (e->Ps[li] - relo_t);
         e->relo_relative_q = Quat::FromR(relo_r.T() * e->Rs[li]);
-        double a = hm::R2ypr(e->Rs[li]).x - hm::R2ypr(relo_r).x;  // Utility::normalizeAngle
-        if (a > 180.0) a -= 360.0;
-        else if (a < -180.0) a += 360.0;
-        e->relo_relative_yaw = a;
+        e->relo_relative_yaw = vb::normalize_angle(vb::R2ypr(e->Rs[li]).x - vb::R2ypr(relo_r).x);  // Utility::normalizeAngle
         e->relocalization_info = false;
         e->fr_relo = false;
         e->n_relo_solves++;
@@ -923,10 +920,10 @@ int stage_frame(ve_estimator* e, bool solve) {
     st.mu = 1e-8;
     // ---- double2vector inputs and the output block
     vb::FinishPlan& fp = q.fin;
-    Vec3 origin_R0 = hm::R2ypr(e->Rs[0]);
+    Vec3 origin_R0 = vb::R2ypr(e->Rs[0]);
     Vec3 origin_P0 = e->Ps[0];
     if (e->failure_occur) {
-        origin_R0 = hm::R2ypr(e->last_R0);
+        origin_R0 = vb::R2ypr(e->last_R0);
         origin_P0 = e->last_P0;
         e->failure_occur = false;
     }

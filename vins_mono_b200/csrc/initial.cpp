@@ -14,43 +14,23 @@ namespace init {
 
 namespace {
 
-inline Vec3 cross(const Vec3& a, const Vec3& b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
-inline double dot(const Vec3& a, const Vec3& b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-inline Mat3 skew(const Vec3& v) {
-    Mat3 m;
-    m(0, 0) = 0; m(0, 1) = -v.z; m(0, 2) = v.y;
-    m(1, 0) = v.z; m(1, 1) = 0; m(1, 2) = -v.x;
-    m(2, 0) = -v.y; m(2, 1) = v.x; m(2, 2) = 0;
-    return m;
-}
-inline Mat3 madd(const Mat3& a, const Mat3& b, double sb = 1.0) {
-    Mat3 r;
-    for (int i = 0; i < 9; i++) r.m[i] = a.m[i] + sb * b.m[i];
-    return r;
-}
-inline Mat3 mscale(const Mat3& a, double s) {
-    Mat3 r;
-    for (int i = 0; i < 9; i++) r.m[i] = a.m[i] * s;
-    return r;
-}
 inline double det3(const Mat3& a) {
     return a(0, 0) * (a(1, 1) * a(2, 2) - a(1, 2) * a(2, 1)) - a(0, 1) * (a(1, 0) * a(2, 2) - a(1, 2) * a(2, 0)) +
            a(0, 2) * (a(1, 0) * a(2, 1) - a(1, 1) * a(2, 0));
 }
-inline Quat qmul(const Quat& a, const Quat& b) {
+// qmul() with the y and z components summed in a different term order
+inline Quat qmul_init(const Quat& a, const Quat& b) {
     return {a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
             a.w * b.y - a.x * b.z + a.y * b.w + a.z * b.x, a.w * b.z + a.x * b.y - a.y * b.x + a.z * b.w};
 }
 inline Quat qconj(const Quat& a) { return {a.w, -a.x, -a.y, -a.z}; }
-inline Vec3 qrot(const Quat& q, const Vec3& v) { return q.R() * v; }
+// q.R() * v, where qrot() is Eigen's quaternion * vector
+inline Vec3 qrot_init(const Quat& q, const Vec3& v) { return q.R() * v; }
 
-// Rodrigues: exp of a rotation vector
+// rodrigues(), except that below |w| = 1e-12 it returns I + [w]x without the [w]x^2 / 2 term
 Mat3 exp_so3(const Vec3& w) {
-    const double th = w.norm();
-    Mat3 I, K = skew(w);
-    if (th < 1e-12) return madd(I, K);
-    const double a = std::sin(th) / th, b = (1 - std::cos(th)) / (th * th);
-    return madd(madd(I, K, a), K * K, b);
+    if (w.norm() < 1e-12) return madd(Mat3(), skew(w));
+    return rodrigues(w);
 }
 
 // Symmetric eigen-decomposition by cyclic Jacobi (n <= 4 here): A (n x n, destroyed) -> eigenvalues in d, vectors in V columns.
@@ -209,15 +189,15 @@ void Preint::start(const Vec3& a0, const Vec3& g0, const Vec3& ba_, const Vec3& 
     valid = true;
 }
 void Preint::propagate(double dt_, const Vec3& a1, const Vec3& g1) {
-    const Vec3 un_acc_0 = qrot(dq, acc_0 - ba);
+    const Vec3 un_acc_0 = qrot_init(dq, acc_0 - ba);
     const Vec3 un_gyr = 0.5 * (gyr_0 + g1) - bg;
-    Quat rq = qmul(dq, Quat(1, un_gyr.x * dt_ / 2, un_gyr.y * dt_ / 2, un_gyr.z * dt_ / 2));
-    const Vec3 un_acc_1 = qrot(rq, a1 - ba);
+    Quat rq = qmul_init(dq, Quat(1, un_gyr.x * dt_ / 2, un_gyr.y * dt_ / 2, un_gyr.z * dt_ / 2));
+    const Vec3 un_acc_1 = qrot_init(rq, a1 - ba);
     const Vec3 un_acc = 0.5 * (un_acc_0 + un_acc_1);
     dp = dp + dv * dt_ + 0.5 * un_acc * dt_ * dt_;
     dv = dv + un_acc * dt_;
     // jacobian = F * jacobian, rows O_R: F(3,3) = I - [w]x dt, F(3,12) = -I dt (integration_base.h:104-105)
-    J_R_bg = madd(madd(Mat3(), skew(un_gyr), -dt_) * J_R_bg, Mat3(), -dt_);
+    J_R_bg = madd(madd(Mat3(), mscale(skew(un_gyr), -dt_)) * J_R_bg, mscale(Mat3(), -dt_));
     dq = rq.normalized();
     sum_dt += dt_;
     acc_0 = a1;
@@ -250,7 +230,7 @@ Vec3 triangulate_point(const double P0[12], const double P1[12], const double x0
         A[8 + c] = x1[0] * P1[8 + c] - P1[0 + c];
         A[12 + c] = x1[1] * P1[8 + c] - P1[4 + c];
     }
-    hm::null_direction4(A, 4, v);
+    null_direction4(A, 4, v);
     return Vec3(v[0] / v[3], v[1] / v[3], v[2] / v[3]);
 }
 
@@ -283,7 +263,7 @@ int recover_pose(const double E[9], const float* p1, const float* p2, int n, uns
                 A[8 + k] = x1[0] * P[8 + k] - P[0 + k];
                 A[12 + k] = x1[1] * P[8 + k] - P[4 + k];
             }
-            hm::null_direction4(A, 4, q);
+            null_direction4(A, 4, q);
             bool ok = q[2] * q[3] > 0;
             const Vec3 X(q[0] / q[3], q[1] / q[3], q[2] / q[3]);
             ok = ok && X.z < dist;
@@ -710,7 +690,7 @@ bool sfm_construct(int frame_num, std::vector<Quat>& q, std::vector<Vec3>& T, in
     }
     q.assign(frame_num, Quat());
     T.assign(frame_num, Vec3());
-    q[frame_num - 1] = qmul(q[l], Quat::FromR(relative_R));
+    q[frame_num - 1] = qmul_init(q[l], Quat::FromR(relative_R));
     T[frame_num - 1] = relative_T;
     std::vector<Mat3> cR(frame_num);
     std::vector<Vec3> cT(frame_num);
@@ -758,7 +738,7 @@ bool sfm_construct(int frame_num, std::vector<Quat>& q, std::vector<Vec3>& T, in
     if (!(conv || cost < 5e-03)) return false;
     for (int i = 0; i < frame_num; i++) {
         q[i] = qconj(Quat::FromR(cR[i]).normalized());
-        T[i] = qrot(q[i], cT[i]) * -1.0;
+        T[i] = qrot_init(q[i], cT[i]) * -1.0;
     }
     for (auto& ft : f)
         if (ft.state) sfm_tracked_points[ft.id] = ft.pos;
@@ -774,7 +754,7 @@ void solve_gyroscope_bias(std::vector<ImageFrame>& fr, std::vector<Vec3>& Bgs, V
         const ImageFrame &fi = fr[i], &fj = fr[i + 1];
         const Quat q_ij = Quat::FromR(fi.R.T() * fj.R);
         const Mat3& J = fj.pre.J_R_bg;
-        const Quat e = qmul(qconj(fj.pre.dq), q_ij);
+        const Quat e = qmul_init(qconj(fj.pre.dq), q_ij);
         const Vec3 tb(2 * e.x, 2 * e.y, 2 * e.z);
         const Mat3 JtJ = J.T() * J;
         const Vec3 Jtb = J.T() * tb;
@@ -1009,8 +989,8 @@ Mat3 g2R(const Vec3& g) {
         q = Quat(s * 0.5, axis.x / s, axis.y / s, axis.z / s);
     }
     Mat3 R0 = q.R();
-    const double yaw = hm::R2ypr(R0).x;
-    return hm::ypr2R(Vec3(-yaw, 0, 0)) * R0;
+    const double yaw = R2ypr(R0).x;
+    return ypr2R(Vec3(-yaw, 0, 0)) * R0;
 }
 
 }  // namespace init
@@ -1079,7 +1059,7 @@ bool ExRotation::calibrate(const std::vector<double>& corres4, const Quat& delta
     for (int i = 1; i <= frame_count; i++) {
         const Quat r1 = Quat::FromR(Rc[i]), r2 = Quat::FromR(Rc_g[i]);
         // Quaterniond::angularDistance: 2 atan2(|vec(d)|, |w(d)|) of d = r1 * r2^-1
-        const Quat dq = qmul(r1, qconj(r2));
+        const Quat dq = qmul_init(r1, qconj(r2));
         const double angular_distance = 180 / M_PI * 2.0 * std::atan2(std::sqrt(dq.x * dq.x + dq.y * dq.y + dq.z * dq.z), std::fabs(dq.w));
         const double huber = angular_distance > 5.0 ? 5.0 / angular_distance : 1.0;
         double L[16], Rm[16];

@@ -9,14 +9,11 @@
 #include <map>
 #include <vector>
 
-#include "host_math.h"
+#include "rotation.h"
 
 namespace vb {
 namespace init {
 
-using hm::Mat3;
-using hm::Quat;
-using hm::Vec3;
 
 // The part of IntegrationBase (factor/integration_base.h:54-186) the initialiser reads: mid-point deltas, sum_dt and
 // d(delta_q)/d(bg).  Samples are kept so that repropagate() can be replayed with a new gyroscope bias.

@@ -6,6 +6,9 @@
 #include "vinsb200/estimator.h"
 
 using namespace vb::init;
+using vb::Mat3;
+using vb::Quat;
+using vb::Vec3;
 
 namespace {
 std::vector<Track> make_tracks(int n, const int* ids, const int* start, const int* nobs, const double* xy) {

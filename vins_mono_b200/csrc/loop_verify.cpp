@@ -16,7 +16,7 @@
 #include "batch_host.h"
 #include "camera_lift.h"
 #include "cuda_check.h"
-#include "host_math.h"
+#include "rotation.h"
 #include "lv_kernels.h"
 #include "lv_layout.h"
 #include "pg_host.h"
@@ -308,9 +308,9 @@ int connect(LvState* s, const int* cur, const int* old, vp_loop_result* r, int c
         rr.n_points = xyid ? (np < cap ? np : cap) : 0;
         for (int i = 0; i < 3; i++) rr.loop_info[i] = o[vb::LV_RES_LOOP + i];
         rr.loop_info[7] = o[vb::LV_RES_LOOP + 7];
-        hm::Mat3 rq;
+        vb::Mat3 rq;
         for (int i = 0; i < 9; i++) rq(i / 3, i % 3) = o[vb::LV_RES_RQ + i];
-        const hm::Quat q = rr.n_inliers ? hm::Quat::FromR(rq) : hm::Quat(1, 0, 0, 0);
+        const vb::Quat q = rr.n_inliers ? vb::Quat::FromR(rq) : vb::Quat(1, 0, 0, 0);
         rr.loop_info[3] = q.w;
         rr.loop_info[4] = q.x;
         rr.loop_info[5] = q.y;

@@ -11,6 +11,7 @@
 #include "camera_lift.h"
 #include "lv_kernels.h"
 #include "lv_layout.h"
+#include "rotation.h"
 
 namespace vb {
 namespace {
@@ -476,22 +477,6 @@ __global__ void __launch_bounds__(HYP_WARPS * 32) lv_pnp_hyp_kernel(const char* 
 
 constexpr int REFIT_THREADS = 128;
 
-__device__ void rodrigues(const double* w, double* R) {
-    const double th = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-    const double a = th < 1e-12 ? 1.0 : sin(th) / th, b = th < 1e-12 ? 0.5 : (1.0 - cos(th)) / (th * th);
-    const double K[9] = {0, -w[2], w[1], w[2], 0, -w[0], -w[1], w[0], 0};
-    for (int i = 0; i < 3; i++)
-        for (int j = 0; j < 3; j++) {
-            double kk = 0;
-            for (int k = 0; k < 3; k++) kk += K[3 * i + k] * K[3 * k + j];
-            R[3 * i + j] = (i == j ? 1.0 : 0.0) + a * K[3 * i + j] + b * kk;
-        }
-}
-
-__device__ double yaw_deg(const double* R) {  // Utility::R2ypr(R).x()
-    return atan2(R[3], R[0]) * (180.0 / 3.14159265358979323846);
-}
-
 // One CTA per job: the best hypothesis (most consensus, lowest index on ties), its consensus set, Gauss-Newton on the
 // reprojection error over that set (float64, fixed-order tree sums), the old key frame's pose and findConnection's gate.
 __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char* arena, const long long* jobs, char* scratch,
@@ -603,10 +588,10 @@ __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char*
                     for (int q = a + 1; q < 6; q++) s -= L[6 * q + a] * d[q];
                     d[a] = s / L[6 * a + a];
                 }
-                double dR[9], R[9];
-                rodrigues(d, dR);
+                const Mat3 dR = rodrigues(Vec3(d[0], d[1], d[2]));
+                double R[9];
                 for (int a = 0; a < 3; a++)
-                    for (int b = 0; b < 3; b++) R[3 * a + b] = dR[3 * a] * P[b] + dR[3 * a + 1] * P[3 + b] + dR[3 * a + 2] * P[6 + b];
+                    for (int b = 0; b < 3; b++) R[3 * a + b] = dR.m[3 * a] * P[b] + dR.m[3 * a + 1] * P[3 + b] + dR.m[3 * a + 2] * P[6 + b];
                 for (int i = 0; i < 9; i++) P[i] = R[i];
                 for (int a = 0; a < 3; a++) P[9 + a] += d[3 + a];
             }
@@ -617,31 +602,24 @@ __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char*
     if (t == 0) {
         // PnP_R_old = R_pnp^T ric^T, PnP_T_old = -R_pnp^T t_pnp - PnP_R_old tic (PnPRANSAC's tail)
         const LvSlotHdr* ch = reinterpret_cast<const LvSlotHdr*>(cur);
-        double Rwc[9], Twc[3], Ro[9], To[3];
+        double Rwc[9], Twc[3], To[3];
+        Mat3 Ro;
         for (int a = 0; a < 3; a++) {
             for (int b = 0; b < 3; b++) Rwc[3 * a + b] = P[3 * b + a];
             Twc[a] = -(P[a] * P[9] + P[3 + a] * P[10] + P[6 + a] * P[11]);
         }
         for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) Ro[3 * a + b] = Rwc[3 * a] * ext_r.v[3 * b] + Rwc[3 * a + 1] * ext_r.v[3 * b + 1] + Rwc[3 * a + 2] * ext_r.v[3 * b + 2];
-        for (int a = 0; a < 3; a++) To[a] = Twc[a] - (Ro[3 * a] * ext_t.v[0] + Ro[3 * a + 1] * ext_t.v[1] + Ro[3 * a + 2] * ext_t.v[2]);
+            for (int b = 0; b < 3; b++) Ro.m[3 * a + b] = Rwc[3 * a] * ext_r.v[3 * b] + Rwc[3 * a + 1] * ext_r.v[3 * b + 1] + Rwc[3 * a + 2] * ext_r.v[3 * b + 2];
+        for (int a = 0; a < 3; a++) To[a] = Twc[a] - (Ro.m[3 * a] * ext_t.v[0] + Ro.m[3 * a + 1] * ext_t.v[1] + Ro.m[3 * a + 2] * ext_t.v[2]);
         // the current key frame's VIO rotation from its quaternion (w x y z)
-        const double qw = ch->vio_Q[0], qx = ch->vio_Q[1], qy = ch->vio_Q[2], qz = ch->vio_Q[3];
-        const double qn = sqrt(qw * qw + qx * qx + qy * qy + qz * qz);
-        const double w_ = qw / qn, x_ = qx / qn, y_ = qy / qn, z_ = qz / qn;
-        const double tx = 2 * x_, ty = 2 * y_, tz = 2 * z_;
-        const double Rc[9] = {1 - (ty * y_ + tz * z_), ty * x_ - tz * w_, tz * x_ + ty * w_,
-                              ty * x_ + tz * w_, 1 - (tx * x_ + tz * z_), tz * y_ - tx * w_,
-                              tz * x_ - ty * w_, tz * y_ + tx * w_, 1 - (tx * x_ + ty * y_)};
+        const Mat3 Rc = Quat(ch->vio_Q[0], ch->vio_Q[1], ch->vio_Q[2], ch->vio_Q[3]).normalized().R();
         double rt[3], rq[9];
         for (int a = 0; a < 3; a++) {
             rt[a] = 0;
-            for (int k = 0; k < 3; k++) rt[a] += Ro[3 * k + a] * (ch->vio_P[k] - To[k]);
-            for (int b = 0; b < 3; b++) rq[3 * a + b] = Ro[a] * Rc[b] + Ro[3 + a] * Rc[3 + b] + Ro[6 + a] * Rc[6 + b];
+            for (int k = 0; k < 3; k++) rt[a] += Ro.m[3 * k + a] * (ch->vio_P[k] - To[k]);
+            for (int b = 0; b < 3; b++) rq[3 * a + b] = Ro.m[a] * Rc.m[b] + Ro.m[3 + a] * Rc.m[3 + b] + Ro.m[6 + a] * Rc.m[6 + b];
         }
-        double yaw = yaw_deg(Rc) - yaw_deg(Ro);
-        if (yaw > 180.0) yaw -= 360.0;
-        else if (yaw < -180.0) yaw += 360.0;
+        const double yaw = normalize_angle(R2ypr(Rc).x - R2ypr(Ro).x);
         const double tn = sqrt(rt[0] * rt[0] + rt[1] * rt[1] + rt[2] * rt[2]);
         const bool accepted = n_in > LV_MIN_LOOP_NUM && fabs(yaw) < 30.0 && tn < 20.0;
         res[0] = accepted;
@@ -649,7 +627,7 @@ __global__ void __launch_bounds__(REFIT_THREADS) lv_pnp_refit_kernel(const char*
         res[3] = n_in;
         for (int a = 0; a < 3; a++) res[LV_RES_LOOP + a] = rt[a];
         res[LV_RES_LOOP + 7] = yaw;
-        for (int i = 0; i < 9; i++) res[LV_RES_R + i] = Ro[i];
+        for (int i = 0; i < 9; i++) res[LV_RES_R + i] = Ro.m[i];
         for (int a = 0; a < 3; a++) res[LV_RES_T + a] = To[a];
         for (int i = 0; i < 9; i++) res[LV_RES_RQ + i] = rq[i];
     }

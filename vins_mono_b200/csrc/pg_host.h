@@ -7,7 +7,7 @@
 
 #include "batch_host.h"
 #include "cuda_check.h"
-#include "host_math.h"
+#include "rotation.h"
 #include "vinsb200/pose_graph.h"
 
 namespace vb {
@@ -26,8 +26,8 @@ int lv_write_points(LvState* s, int member, int first, const std::vector<MapKeyF
 
 struct PgKeyFrame {
     double stamp = 0;
-    hm::Vec3 vio_P, P;
-    hm::Mat3 vio_R, R;
+    Vec3 vio_P, P;
+    Mat3 vio_R, R;
     int seq = 0;
     bool has_loop = false;
     int loop_index = -1;
@@ -41,8 +41,8 @@ struct vp_graph : vb::MemberBase<vp_batch> {
     int sequence = 1;      // the node's sequence counter (pose_graph_node.cpp:69-72)
     int sequence_cnt = 0;  // PoseGraph::sequence_cnt
     std::vector<int> sequence_loop{0};
-    hm::Mat3 w_r_vio, r_drift;
-    hm::Vec3 w_t_vio, t_drift;
+    vb::Mat3 w_r_vio, r_drift;
+    vb::Vec3 w_t_vio, t_drift;
     double yaw_drift = 0;
     int earliest_loop_index = -1, pending = -1, n_loops = 0, n_opt = 0;
     int n_map = 0;  // key frames 0 .. n_map - 1 came from vp_load: sequence 0, constant in every optimisation

@@ -41,14 +41,7 @@
 namespace vb {
 namespace {
 
-constexpr double PG_PI = 3.14159265358979323846;
 constexpr double PG_HUBER_A = 0.1;  // HuberLoss(0.1), pose_graph.cpp:440
-
-__device__ __forceinline__ double normalize_angle(double a) {  // NormalizeAngle, pose_graph.h:89-97
-    if (a > 180.0) return a - 360.0;
-    if (a < -180.0) return a + 360.0;
-    return a;
-}
 
 // FourDOFError / FourDOFWeightError (pose_graph.h:159-248) between the older key frame i (yaw_i, pitch_i, roll_i) and the
 // newer j; xi / xj = yaw (degrees), t.  meas = t_rel (3), yaw_rel.  J (may be NULL): 4 x 8, columns yaw_i, t_i, yaw_j,
@@ -56,13 +49,13 @@ __device__ __forceinline__ double normalize_angle(double a) {  // NormalizeAngle
 // sqrt(rho')) is applied.  Returns the cost 0.5 rho(|r|^2).
 __device__ double four_dof_eval(const double* xi, const double* xj, double pitch_i, double roll_i, const double* meas, bool weighted,
                                 bool robust, double* r, double* J) {
-    const M3d R = ypr2R_dev(mk(xi[0], pitch_i, roll_i));
+    const Mat3 R = ypr2R(Vec3(xi[0], pitch_i, roll_i));
     const double d0 = xj[1] - xi[1], d1 = xj[2] - xi[2], d2 = xj[3] - xi[3];
     for (int k = 0; k < 3; k++) r[k] = (R.m[k] * d0 + R.m[3 + k] * d1 + R.m[6 + k] * d2) - meas[k];
     r[3] = normalize_angle(xj[0] - xi[0] - meas[3]);
     if (weighted) r[3] = r[3] / 10.0;
     if (J) {
-        const double c = PG_PI / 180.0, w = weighted ? 0.1 : 1.0;
+        const double c = M_PI / 180.0, w = weighted ? 0.1 : 1.0;
         // dR/dyaw = [[0,-1,0],[1,0,0],[0,0,0]] R: row 0 = -R row 1, row 1 = R row 0
         for (int k = 0; k < 3; k++) {
             J[8 * k] = c * (-R.m[3 + k] * d0 + R.m[k] * d1);
@@ -186,7 +179,7 @@ __global__ void __launch_bounds__(256) pg_setup_kernel(PgLaunch a) {
     const PgView v = pg_view(a, blockIdx.x);
     for (int k = threadIdx.x; k < v.n; k += blockDim.x) {
         const double* p = v.pose + 7 * k;
-        const V3d ypr = R2ypr_dev(qR(Q4{p[3], p[4], p[5], p[6]}));
+        const Vec3 ypr = R2ypr(qR(Quat{p[3], p[4], p[5], p[6]}));
         v.ypr[3 * k] = ypr.x; v.ypr[3 * k + 1] = ypr.y; v.ypr[3 * k + 2] = ypr.z;
         v.x[4 * k] = ypr.x; v.x[4 * k + 1] = p[0]; v.x[4 * k + 2] = p[1]; v.x[4 * k + 3] = p[2];
     }
@@ -197,7 +190,7 @@ __global__ void __launch_bounds__(256) pg_setup_kernel(PgLaunch a) {
             double* m = v.smeas + 16 * k + 4 * e;
             if (b < 0) { m[0] = m[1] = m[2] = m[3] = 0.0; continue; }
             const double* pb = v.pose + 7 * b;
-            const M3d Rb = qR(Q4{pb[3], pb[4], pb[5], pb[6]});
+            const Mat3 Rb = qR(Quat{pb[3], pb[4], pb[5], pb[6]});
             const double d0 = v.x[4 * k + 1] - v.x[4 * b + 1], d1 = v.x[4 * k + 2] - v.x[4 * b + 2], d2 = v.x[4 * k + 3] - v.x[4 * b + 3];
             for (int c = 0; c < 3; c++) m[c] = Rb.m[c] * d0 + Rb.m[3 + c] * d1 + Rb.m[6 + c] * d2;
             m[3] = v.x[4 * k] - v.x[4 * b];

@@ -14,15 +14,15 @@
 
 #include "batch_host.h"
 #include "cuda_check.h"
-#include "host_math.h"
+#include "rotation.h"
 #include "pg_host.h"
 #include "pg_kernels.h"
 #include "pg_layout.h"
 #include "pg_map.h"
 
-using hm::Mat3;
-using hm::Quat;
-using hm::Vec3;
+using vb::Mat3;
+using vb::Quat;
+using vb::Vec3;
 using KeyFrame = vb::PgKeyFrame;
 
 namespace {
@@ -33,7 +33,7 @@ bool loop_gate(const double* li) {  // keyframe.cpp:480, :573
     return std::fabs(li[7]) < 30.0 && Vec3(li[0], li[1], li[2]).norm() < 20.0;
 }
 
-Mat3 yaw_R(double yaw) { return hm::ypr2R(Vec3(yaw, 0, 0)); }
+Mat3 yaw_R(double yaw) { return vb::ypr2R(Vec3(yaw, 0, 0)); }
 
 // Waits for the batch's launch in flight and copies each member's output block to the member (not yet applied).
 int batch_wait(vp_batch* b) {
@@ -76,17 +76,17 @@ int collect(vp_graph* g) {
     for (int i = 0; i < n; i++) {
         KeyFrame& kf = g->kfs[g->inf_map[i]];
         if (kf.seq == 0) continue;
-        kf.R = hm::ypr2R(Vec3(o[4 * i], g->inf_pr[2 * i], g->inf_pr[2 * i + 1]));
+        kf.R = vb::ypr2R(Vec3(o[4 * i], g->inf_pr[2 * i], g->inf_pr[2 * i + 1]));
         kf.P = Vec3(o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
     }
     // the loaded map's key frames of the range, packed or not: updatePose(t, ypr2R(euler)) of a constant block
     for (int k = first; k < g->n_map; k++) {
         KeyFrame& kf = g->kfs[k];
-        kf.R = hm::ypr2R(hm::R2ypr(Quat::FromR(kf.vio_R).R()));
+        kf.R = vb::ypr2R(vb::R2ypr(Quat::FromR(kf.vio_R).R()));
         kf.P = kf.vio_P;
     }
     const KeyFrame& ck = g->kfs[cur];
-    g->yaw_drift = hm::R2ypr(ck.R).x - hm::R2ypr(ck.vio_R).x;
+    g->yaw_drift = vb::R2ypr(ck.R).x - vb::R2ypr(ck.vio_R).x;
     g->r_drift = yaw_R(g->yaw_drift);
     g->t_drift = ck.P - g->r_drift * ck.vio_P;
     for (size_t k = cur + 1; k < g->kfs.size(); k++) {
@@ -172,7 +172,7 @@ int pack_member(vp_graph* g, char* base, size_t off, int* n_out, int* nb_out, in
         const Quat q = Quat::FromR(kf.vio_R);
         const double p[7] = {kf.vio_P.x, kf.vio_P.y, kf.vio_P.z, q.w, q.x, q.y, q.z};
         std::memcpy(pose + 7 * i, p, sizeof(p));
-        const Vec3 ypr = hm::R2ypr(q.R());
+        const Vec3 ypr = vb::R2ypr(q.R());
         (*pr)[2 * i] = ypr.y;
         (*pr)[2 * i + 1] = ypr.z;
         seq[i] = packed_edges ? kf.seq : -1 - i;
@@ -358,7 +358,7 @@ int vp_add_keyframe(vp_graph* g, double stamp, const double* vio_P3, const doubl
         const Mat3 rel_R = Quat(loop_info8[3], loop_info8[4], loop_info8[5], loop_info8[6]).R();
         const Vec3 w_P_cur = old.vio_R * rel_t + old.vio_P;
         const Mat3 w_R_cur = old.vio_R * rel_R;
-        const double shift_yaw = hm::R2ypr(w_R_cur).x - hm::R2ypr(kf.vio_R).x;
+        const double shift_yaw = vb::R2ypr(w_R_cur).x - vb::R2ypr(kf.vio_R).x;
         const Mat3 shift_r = yaw_R(shift_yaw);
         const Vec3 shift_t = w_P_cur - w_R_cur * kf.vio_R.T() * kf.vio_P;
         if (old.seq != kf.seq && g->sequence_loop[kf.seq] == 0) {  // pose_graph.cpp:96-124
@@ -399,7 +399,7 @@ int vp_update_loop(vp_graph* g, int index, const double* loop_info8) {
         const Mat3 rel_R = Quat(loop_info8[3], loop_info8[4], loop_info8[5], loop_info8[6]).R();
         const Vec3 w_P_cur = old.R * rel_t + old.P;
         const Mat3 w_R_cur = old.R * rel_R;
-        g->yaw_drift = hm::R2ypr(w_R_cur).x - hm::R2ypr(kf.vio_R).x;
+        g->yaw_drift = vb::R2ypr(w_R_cur).x - vb::R2ypr(kf.vio_R).x;
         g->r_drift = yaw_R(g->yaw_drift);
         g->t_drift = w_P_cur - w_R_cur * kf.vio_R.T() * kf.vio_P;
     }

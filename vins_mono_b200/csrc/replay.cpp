@@ -7,7 +7,7 @@
 #include <cstdio>
 #include <cstring>
 
-#include "host_math.h"
+#include "rotation.h"
 
 #include <atomic>
 #include <condition_variable>
@@ -452,23 +452,12 @@ int vr_debug_imu_batches(int n_imu, const double* imu_t, const double* acc, cons
 
 struct vr_propagator {  // the globals of estimator_node.cpp:21-40
     double latest_time = 0;
-    hm::Vec3 tmp_P, tmp_V, tmp_Ba, tmp_Bg, acc_0, gyr_0, g;
-    hm::Quat tmp_Q;
+    vb::Vec3 tmp_P, tmp_V, tmp_Ba, tmp_Bg, acc_0, gyr_0, g;
+    vb::Quat tmp_Q;
     bool init_imu = true;
 };
 
 namespace {
-hm::Quat qmul(const hm::Quat& a, const hm::Quat& b) {
-    return hm::Quat(a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-                    a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z, a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x);
-}
-hm::Vec3 qrot(const hm::Quat& q, const hm::Vec3& v) {  // Eigen's quaternion * vector
-    const hm::Vec3 u(q.x, q.y, q.z);
-    auto cross = [](const hm::Vec3& a, const hm::Vec3& b) { return hm::Vec3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); };
-    hm::Vec3 uv = cross(u, v);
-    uv = uv + uv;
-    return v + uv * q.w + cross(u, uv);
-}
 void prop_one(vr_propagator* p, double t, const double* a, const double* w) {
     if (p->init_imu) {
         p->latest_time = t;
@@ -477,12 +466,12 @@ void prop_one(vr_propagator* p, double t, const double* a, const double* w) {
     }
     const double dt = t - p->latest_time;
     p->latest_time = t;
-    const hm::Vec3 acc(a[0], a[1], a[2]), gyr(w[0], w[1], w[2]);
-    const hm::Vec3 un_acc_0 = qrot(p->tmp_Q, p->acc_0 - p->tmp_Ba) - p->g;
-    const hm::Vec3 un_gyr = 0.5 * (p->gyr_0 + gyr) - p->tmp_Bg;
-    p->tmp_Q = qmul(p->tmp_Q, hm::Quat(1.0, un_gyr.x * dt / 2.0, un_gyr.y * dt / 2.0, un_gyr.z * dt / 2.0));  // Utility::deltaQ, not normalised
-    const hm::Vec3 un_acc_1 = qrot(p->tmp_Q, acc - p->tmp_Ba) - p->g;
-    const hm::Vec3 un_acc = 0.5 * (un_acc_0 + un_acc_1);
+    const vb::Vec3 acc(a[0], a[1], a[2]), gyr(w[0], w[1], w[2]);
+    const vb::Vec3 un_acc_0 = vb::qrot(p->tmp_Q, p->acc_0 - p->tmp_Ba) - p->g;
+    const vb::Vec3 un_gyr = 0.5 * (p->gyr_0 + gyr) - p->tmp_Bg;
+    p->tmp_Q = vb::qmul(p->tmp_Q, vb::deltaQ(un_gyr * dt));
+    const vb::Vec3 un_acc_1 = vb::qrot(p->tmp_Q, acc - p->tmp_Ba) - p->g;
+    const vb::Vec3 un_acc = 0.5 * (un_acc_0 + un_acc_1);
     p->tmp_P = p->tmp_P + dt * p->tmp_V + 0.5 * dt * dt * un_acc;
     p->tmp_V = p->tmp_V + dt * un_acc;
     p->acc_0 = acc;
@@ -513,14 +502,14 @@ int vr_prop_update(vr_propagator* p, double current_time, const double* P3, cons
                    const double* gyr) {
     if (!p || !P3 || !Q || !V3 || !Ba3 || !Bg3 || !acc0 || !gyr0 || !g3 || n < 0 || (n && (!t || !acc || !gyr))) return -1;
     p->latest_time = current_time;
-    p->tmp_P = hm::Vec3(P3[0], P3[1], P3[2]);
-    p->tmp_Q = hm::Quat(Q[0], Q[1], Q[2], Q[3]);
-    p->tmp_V = hm::Vec3(V3[0], V3[1], V3[2]);
-    p->tmp_Ba = hm::Vec3(Ba3[0], Ba3[1], Ba3[2]);
-    p->tmp_Bg = hm::Vec3(Bg3[0], Bg3[1], Bg3[2]);
-    p->acc_0 = hm::Vec3(acc0[0], acc0[1], acc0[2]);
-    p->gyr_0 = hm::Vec3(gyr0[0], gyr0[1], gyr0[2]);
-    p->g = hm::Vec3(g3[0], g3[1], g3[2]);
+    p->tmp_P = vb::Vec3(P3[0], P3[1], P3[2]);
+    p->tmp_Q = vb::Quat(Q[0], Q[1], Q[2], Q[3]);
+    p->tmp_V = vb::Vec3(V3[0], V3[1], V3[2]);
+    p->tmp_Ba = vb::Vec3(Ba3[0], Ba3[1], Ba3[2]);
+    p->tmp_Bg = vb::Vec3(Bg3[0], Bg3[1], Bg3[2]);
+    p->acc_0 = vb::Vec3(acc0[0], acc0[1], acc0[2]);
+    p->gyr_0 = vb::Vec3(gyr0[0], gyr0[1], gyr0[2]);
+    p->g = vb::Vec3(g3[0], g3[1], g3[2]);
     for (int k = 0; k < n; k++) prop_one(p, t[k], acc + 3 * k, gyr + 3 * k);
     return 0;
 }
@@ -578,7 +567,7 @@ int vr_decode_relo_message(int n, const float* xyz, const float* channel0_values
     const float* c = channel0_values8;
     for (int k = 0; k < 3; k++) relo_t3[k] = c[k];
     // Quaterniond relo_q(values[3], values[4], values[5], values[6]) = (w, x, y, z); toRotationMatrix() does not normalise
-    const hm::Mat3 R = hm::Quat(c[3], c[4], c[5], c[6]).R();
+    const vb::Mat3 R = vb::Quat(c[3], c[4], c[5], c[6]).R();
     std::memcpy(relo_r9, R.m, sizeof(R.m));
     if (frame_index) *frame_index = (int)c[7];
     return n;
