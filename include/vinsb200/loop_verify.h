@@ -15,7 +15,8 @@
  *                            n window points (point_3d, point_2d_uv, point_2d_norm, point_id).  GaussianBlur 9x9 sigma 2,
  *                            FAST-9 (threshold 20, non-max suppression), BRIEF on both point sets and liftProjective of the
  *                            corners run on the device; the call returns once the slot is written.  n > max_window or more
- *                            corners than max_corners is VP_ERR_CAPACITY and leaves the slot as it was.
+ *                            corners than max_corners is VP_ERR_CAPACITY and leaves the slot as it was.  It is a one-job
+ *                            vp_batch_attach_keyframes (loop_attach.h), which attaches many key frames in one launch chain.
  *   vp_find_connection       findConnection(old) for two attached slots: Hamming matching (best < 80, the first index of the
  *                            smallest distance), more than 25 matches, PnP-RANSAC (float64, see DESIGN §5: not OpenCV's
  *                            sampler or solver), more than 25 inliers, |relative_yaw| < 30 and |relative_t| < 20.
@@ -23,8 +24,8 @@
  *                            order: ve_set_relo_frame's match_points.
  *   vp_batch_find_connection one launch chain for every member k with cur[k] >= 0 (results r[k], lists at
  *                            match_xyid + 3 cap k); status[k] (may be NULL) 1 = verified, 0 = skipped, < 0 error.
- *   vp_loop_last_timing      device ms (CUDA events) of the last attach (blur, FAST, BRIEF) and of the last verification
- *                            launch chain (matching, hypotheses, refit).
+ *   vp_loop_last_timing      device ms (CUDA events) of the last attach call (blur, FAST, BRIEF; all its jobs) and of
+ *                            the last verification launch chain (matching, hypotheses, refit).
  *
  * A key frame loaded by vp_load (pose_graph.h) has a slot with its saved corners and descriptors and no window points:
  * it can be `old` of vp_find_connection; as `cur` it matches nothing.

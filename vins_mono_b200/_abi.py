@@ -41,6 +41,12 @@ class LoopResult(C.Structure):  # vp_loop_result
                 ("loop_info", C.c_double * 8), ("old_R9", C.c_double * 9), ("old_T3", C.c_double * 3)]
 
 
+class AttachJob(C.Structure):  # vp_attach_job
+    _fields_ = [("member", C.c_int), ("index", C.c_int), ("vio_P3", C.c_void_p), ("vio_Qwxyz", C.c_void_p), ("img", C.c_void_p),
+                ("row_stride", C.c_size_t), ("img_on_device", C.c_int), ("n", C.c_int), ("point_3d", C.c_void_p),
+                ("point_uv", C.c_void_p), ("point_norm", C.c_void_p), ("point_id", C.c_void_p)]
+
+
 class ReplaySequence(C.Structure):  # vr_sequence
     _fields_ = [("images", C.c_void_p), ("row_stride", C.c_size_t), ("frame_stride", C.c_size_t), ("n_images", C.c_int),
                 ("images_on_device", C.c_int), ("stamps", C.c_void_p), ("n_imu", C.c_int), ("imu_t", C.c_void_p),
@@ -169,6 +175,8 @@ SIGNATURES = {
     "vp_debug_brief": (I, [V, I, I, V, I, V, V]),
     "vp_debug_match": (I, [I, V, I, V, V]),
     "vp_debug_pnp": (I, [I, V, V, V, IP, V]),
+    # loop_attach.h
+    "vp_batch_attach_keyframes": (I, [V, I, V, V, V]),
     # loop_camera.h
     "vp_loop_enable_camera": (I, [V, C.POINTER(LoopConfig), I, D]),
     "vp_batch_loop_enable_camera": (I, [V, C.POINTER(LoopConfig), I, D]),

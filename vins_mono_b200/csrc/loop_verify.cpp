@@ -2,6 +2,7 @@
 // key-frame attach and the verification of candidate pairs around the device stages of lv_kernels.cu.
 #include "vinsb200/loop_verify.h"
 
+#include "vinsb200/loop_attach.h"
 #include "vinsb200/loop_camera.h"
 #include "vinsb200/tracker.h"
 
@@ -36,7 +37,8 @@ struct LvState {
     double xi = 0.0;
     int pattern[4 * LV_BITS] = {};
     int S = 0, cap_kf = 0, device = 0;
-    size_t slot_bytes = 0, stage_bytes = 0, conn_bytes = 0, res_doubles = 0;
+    size_t slot_bytes = 0, stage_bytes = 0, ascratch_bytes = 0, conn_bytes = 0, res_doubles = 0;
+    int attach_cap = 0;  // jobs the attach buffers hold: the packed stage, the attach scratch and the status
     DeviceArray<char> d_arena, d_stage, d_ascratch, d_cscratch;
     PinnedArray<char> h_stage;
     DeviceArray<int> d_pattern;
@@ -147,10 +149,11 @@ int create_resources(LvState* s, std::string* err) {
     const size_t arena = vb::lv_arena_bytes(s->S, s->cap_kf, c->max_window, c->max_corners);
     VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_arena.alloc(arena));
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemset(s->d_arena, 0, arena));
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_stage.alloc(s->stage_bytes));
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_stage.alloc(s->stage_bytes));
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_ascratch.alloc(vb::lv_attach_layout(c->rows, c->cols).total));
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_status.alloc(4));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_stage.alloc(vb::lv_attach_jobs_bytes(1) + s->stage_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_stage.alloc(vb::lv_attach_jobs_bytes(1) + s->stage_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_ascratch.alloc(s->ascratch_bytes));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, s->h_status.alloc(2));
+    s->attach_cap = 1;
     VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_cscratch.alloc(S * s->conn_bytes));
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemset(s->d_cscratch, 0, S * s->conn_bytes));
     VB_CUDA_CHECK(err, VP_ERR_CUDA, s->d_pattern.alloc(4 * vb::LV_BITS));
@@ -182,6 +185,7 @@ int enable(LvState** slot, const vp_loop_config* c, int camera_model, double xi,
     s->device = device;
     s->slot_bytes = vb::lv_slot_layout(c->max_window, c->max_corners).total;
     s->stage_bytes = vb::lv_stage_layout(c->rows, c->cols, c->max_window).total;
+    s->ascratch_bytes = vb::lv_attach_layout(c->rows, c->cols).total;
     s->conn_bytes = vb::lv_conn_layout(c->max_window).total;
     s->res_doubles = vb::lv_result_doubles(c->max_window);
     s->attached.assign((size_t)S * cap_kf, 0);
@@ -201,58 +205,135 @@ int drain_on_error(LvState* s, int rc) {
     return rc;
 }
 
-// One staged key frame into arena slot `slot`: the input copy, the attach chain, the status copy, then a wait.
-int attach_chain(LvState* s, size_t slot, std::string* err) {
-    const vp_loop_config& c = s->cfg;
+// The attach buffers grown to hold n jobs.  New buffers are allocated before the old ones go (the stream is idle between
+// calls), so a failure leaves the state as it was: VP_ERR_CAPACITY.
+int reserve_attach(LvState* s, int n, std::string* err) {
+    if (n <= s->attach_cap) return 0;
+    const size_t stage = vb::lv_attach_jobs_bytes(n) + (size_t)n * s->stage_bytes;
+    vb::DeviceArray<char> d_stage, d_scratch;
+    vb::PinnedArray<char> h_stage;
+    vb::PinnedArray<int> h_status;
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_stage, s->h_stage, s->stage_bytes, cudaMemcpyHostToDevice, s->stream));
-    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, s->d_arena + slot * s->slot_bytes, s->d_pattern,
+    if (d_stage.alloc(stage) || h_stage.alloc(stage) || d_scratch.alloc((size_t)n * s->ascratch_bytes) || h_status.alloc(2 * (size_t)n)) {
+        cudaGetLastError();
+        *err = "vp_batch_attach_keyframes: the staging buffers of " + std::to_string(n) + " jobs do not fit in memory";
+        return VP_ERR_CAPACITY;
+    }
+    s->d_stage = std::move(d_stage);
+    s->h_stage = std::move(h_stage);
+    s->d_ascratch = std::move(d_scratch);
+    s->h_status = std::move(h_status);
+    s->attach_cap = n;
+    return 0;
+}
+
+// The staged jobs into their slots: the packed-stage copy, one copy per device image, the attach chain over every job,
+// the status copy, then a wait.
+int attach_chain(LvState* s, int n, const vp_attach_job* jobs, std::string* err) {
+    const vp_loop_config& c = s->cfg;
+    const size_t jb = vb::lv_attach_jobs_bytes(n);
+    char* d_blocks = s->d_stage + jb;
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaSetDevice(s->device));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_stage, s->h_stage, jb + (size_t)n * s->stage_bytes, cudaMemcpyHostToDevice, s->stream));
+    const size_t img = vb::lv_stage_layout(c.rows, c.cols, c.max_window).img;
+    for (int j = 0; j < n; j++) {
+        if (!jobs[j].img_on_device) continue;
+        VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy2DAsync(d_blocks + (size_t)j * s->stage_bytes + img, c.cols, jobs[j].img, jobs[j].row_stride,
+                                                          c.cols, c.rows, cudaMemcpyDeviceToDevice, s->stream));
+    }
+    vb::LvAttachLaunch L{d_blocks, s->d_ascratch, s->d_arena, reinterpret_cast<const long long*>(s->d_stage.get()), n, s->d_pattern,
                          c.rows, c.cols, c.max_window, c.max_corners, {}, s->camera_model, s->xi};
     std::memcpy(L.intrinsics, c.intrinsics, sizeof(L.intrinsics));
     cudaEvent_t ev[4] = {s->ev[0], s->ev[1], s->ev[2], s->ev[3]};
     vb::launch_lv_attach(L, s->stream, ev);
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaGetLastError());
-    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpyAsync(s->h_status, s->d_ascratch + vb::lv_attach_layout(c.rows, c.cols).status, 8,
-                                                    cudaMemcpyDeviceToHost, s->stream));
+    VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaMemcpy2DAsync(s->h_status, 8, s->d_ascratch + vb::lv_attach_layout(c.rows, c.cols).status,
+                                                      s->ascratch_bytes, 8, n, cudaMemcpyDeviceToHost, s->stream));
     VB_CUDA_CHECK(err, VP_ERR_CUDA, cudaStreamSynchronize(s->stream));
     for (int k = 0; k < 3; k++) cudaEventElapsedTime(&s->ms[k], s->ev[k], s->ev[k + 1]);
     return 0;
 }
 
-int attach(LvState* s, int member, int index, const double* P3, const double* Q4, const uint8_t* img, size_t stride, int n,
-           const float* p3d, const float* uv, const float* norm, const double* ids, int* n_corners, std::string* err) {
+// n_jobs key frames into their slots in one launch chain.  single: the call is vp_attach_keyframe, whose texts name no
+// job and for which more window points than max_window is VP_ERR_CAPACITY (a batch call: VP_ERR_INVALID).
+int attach(LvState* s, int n_jobs, const vp_attach_job* jobs, int* n_corners, int* status, bool single, std::string* err) {
     const vp_loop_config& c = s->cfg;
-    if (index < 0 || index >= s->cap_kf || !P3 || !Q4 || !img || stride < (size_t)c.cols || n < 0 ||
-        (n > 0 && (!p3d || !uv || !norm || !ids))) {
-        *err = "vp_attach_keyframe: invalid argument";
+    const char* fn = single ? "vp_attach_keyframe" : "vp_batch_attach_keyframes";
+    const auto job_text = [&](int j) { return std::string(fn) + ": " + (single ? "" : "job " + std::to_string(j) + ": "); };
+    if (n_jobs < 0 || (n_jobs && !jobs)) {
+        *err = std::string(fn) + ": invalid argument";
         return VP_ERR_INVALID;
     }
-    if (n > c.max_window) {
-        *err = "vp_attach_keyframe: " + std::to_string(n) + " window points, at most max_window = " + std::to_string(c.max_window);
+    if (status)
+        for (int j = 0; j < n_jobs; j++) status[j] = 0;
+    std::vector<char> seen((size_t)s->S * s->cap_kf, 0);
+    for (int j = 0; j < n_jobs; j++) {
+        const vp_attach_job& a = jobs[j];
+        int rc = 0;
+        if (a.member < 0 || a.member >= s->S || a.index < 0 || a.index >= s->cap_kf || !a.vio_P3 || !a.vio_Qwxyz || !a.img ||
+            a.row_stride < (size_t)c.cols || a.n < 0 || (a.n > 0 && (!a.point_3d || !a.point_uv || !a.point_norm || !a.point_id))) {
+            *err = job_text(j) + "invalid argument";
+            rc = VP_ERR_INVALID;
+        } else if (a.n > c.max_window) {
+            *err = job_text(j) + std::to_string(a.n) + " window points, at most max_window = " + std::to_string(c.max_window);
+            rc = single ? VP_ERR_CAPACITY : VP_ERR_INVALID;
+        } else if (seen[(size_t)a.member * s->cap_kf + a.index]++) {
+            *err = job_text(j) + "member " + std::to_string(a.member) + " slot " + std::to_string(a.index) + " appears twice";
+            rc = VP_ERR_INVALID;
+        }
+        if (!rc) continue;
+        if (status) status[j] = rc;
+        return rc;
+    }
+    if (!n_jobs) return 0;
+    if (n_jobs > 65535) {  // gridDim.z
+        *err = std::string(fn) + ": " + std::to_string(n_jobs) + " jobs, at most 65535 in one call";
         return VP_ERR_CAPACITY;
     }
+    if (const int rc = reserve_attach(s, n_jobs, err)) return rc;
     const vb::LvStageLayout st = vb::lv_stage_layout(c.rows, c.cols, c.max_window);
-    vb::LvSlotHdr h{};
-    std::memcpy(h.vio_P, P3, sizeof(h.vio_P));
-    std::memcpy(h.vio_Q, Q4, sizeof(h.vio_Q));
-    h.n_win = n;
-    std::memcpy(s->h_stage, &h, sizeof(h));
-    for (int y = 0; y < c.rows; y++) std::memcpy(s->h_stage + st.img + (size_t)y * c.cols, img + (size_t)y * stride, c.cols);
-    if (n) {
-        std::memcpy(s->h_stage + st.p3d, p3d, 12 * (size_t)n);
-        std::memcpy(s->h_stage + st.uv, uv, 8 * (size_t)n);
-        std::memcpy(s->h_stage + st.norm, norm, 8 * (size_t)n);
-        std::memcpy(s->h_stage + st.id, ids, 8 * (size_t)n);
+    long long* slots = reinterpret_cast<long long*>(s->h_stage.get());
+    for (int j = 0; j < n_jobs; j++) {
+        const vp_attach_job& a = jobs[j];
+        char* blk = s->h_stage + vb::lv_attach_jobs_bytes(n_jobs) + (size_t)j * s->stage_bytes;
+        slots[j] = (long long)(((size_t)a.member * s->cap_kf + a.index) * s->slot_bytes);
+        vb::LvSlotHdr h{};
+        std::memcpy(h.vio_P, a.vio_P3, sizeof(h.vio_P));
+        std::memcpy(h.vio_Q, a.vio_Qwxyz, sizeof(h.vio_Q));
+        h.n_win = a.n;
+        std::memcpy(blk, &h, sizeof(h));
+        if (!a.img_on_device)
+            for (int y = 0; y < c.rows; y++) std::memcpy(blk + st.img + (size_t)y * c.cols, a.img + (size_t)y * a.row_stride, c.cols);
+        if (a.n) {
+            std::memcpy(blk + st.p3d, a.point_3d, 12 * (size_t)a.n);
+            std::memcpy(blk + st.uv, a.point_uv, 8 * (size_t)a.n);
+            std::memcpy(blk + st.norm, a.point_norm, 8 * (size_t)a.n);
+            std::memcpy(blk + st.id, a.point_id, 8 * (size_t)a.n);
+        }
     }
-    const int rc = drain_on_error(s, attach_chain(s, (size_t)member * s->cap_kf + index, err));
+    const int rc = drain_on_error(s, attach_chain(s, n_jobs, jobs, err));
     if (rc) return rc;
-    if (n_corners) *n_corners = s->h_status[0];
-    if (s->h_status[1]) {
-        *err = "vp_attach_keyframe: " + std::to_string(s->h_status[0]) + " FAST corners, at most max_corners = " + std::to_string(c.max_corners);
-        return VP_ERR_CAPACITY;
+    int first_over = -1;
+    for (int j = 0; j < n_jobs; j++) {
+        if (n_corners) n_corners[j] = s->h_status[2 * j];
+        if (s->h_status[2 * j + 1]) {
+            if (status) status[j] = VP_ERR_CAPACITY;
+            if (first_over < 0) first_over = j;
+            continue;
+        }
+        s->attached[(size_t)jobs[j].member * s->cap_kf + jobs[j].index] = 1;
     }
-    s->attached[(size_t)member * s->cap_kf + index] = 1;
-    return 0;
+    if (first_over < 0) return 0;
+    *err = job_text(first_over) + std::to_string(s->h_status[2 * first_over]) + " FAST corners, at most max_corners = " +
+           std::to_string(c.max_corners);
+    return VP_ERR_CAPACITY;
+}
+
+// vp_attach_keyframe's arguments as the one job of an attach call.
+int attach_one(LvState* s, int member, int index, const double* P3, const double* Q4, const uint8_t* img, size_t stride, int n,
+               const float* p3d, const float* uv, const float* norm, const double* ids, int* n_corners, std::string* err) {
+    const vp_attach_job job{member, index, P3, Q4, img, stride, 0, n, p3d, uv, norm, ids};
+    return attach(s, 1, &job, n_corners, nullptr, true, err);
 }
 
 // The job copy, the verification chain of `jobs` pairs, the result copy, then a wait.
@@ -380,8 +461,18 @@ int vp_attach_keyframe(vp_graph* g, int index, const double* vio_P3, const doubl
         g->err = "vp_attach_keyframe: loop verification is not enabled";
         return VP_ERR_INVALID;
     }
-    return attach(s, g->member, index, vio_P3, vio_Qwxyz, img, row_stride, n, point_3d, point_uv, point_norm, point_id, n_corners,
-                  &g->err);
+    return attach_one(s, g->member, index, vio_P3, vio_Qwxyz, img, row_stride, n, point_3d, point_uv, point_norm, point_id, n_corners,
+                      &g->err);
+}
+
+int vp_batch_attach_keyframes(vp_batch* b, int n_jobs, const vp_attach_job* jobs, int* n_corners, int* status) {
+    if (!b) return VP_ERR_INVALID;
+    LvState* s = b->lv;
+    if (!s) {
+        b->err = "vp_batch_attach_keyframes: loop verification is not enabled";
+        return VP_ERR_INVALID;
+    }
+    return attach(s, n_jobs, jobs, n_corners, status, false, &b->err);
 }
 
 int vp_find_connection(vp_graph* g, int cur, int old, vp_loop_result* r, int cap, double* match_xyid) {
@@ -434,7 +525,7 @@ int vp_debug_brief_blur(const uint8_t* img, int rows, int cols, uint8_t* out) {
     DebugState d(rows, cols, nullptr, 1, vb::LV_CAP_CORNERS);
     if (d.rc) return d.rc;
     int nc = 0;
-    int rc = attach(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, 0, nullptr, nullptr, nullptr, nullptr, &nc, &d.err);
+    int rc = attach_one(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, 0, nullptr, nullptr, nullptr, nullptr, &nc, &d.err);
     if (rc && rc != VP_ERR_CAPACITY) return rc;
     return cudaMemcpy(out, d.s->d_ascratch + vb::lv_attach_layout(rows, cols).blur, (size_t)rows * cols, cudaMemcpyDeviceToHost) == cudaSuccess
                ? 0 : VP_ERR_CUDA;
@@ -445,7 +536,7 @@ int vp_debug_fast(const uint8_t* img, int rows, int cols, int cap, float* xy) {
     DebugState d(rows, cols, nullptr, 1, cap);
     if (d.rc) return d.rc;
     int nc = 0;
-    const int rc = attach(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, 0, nullptr, nullptr, nullptr, nullptr, &nc, &d.err);
+    const int rc = attach_one(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, 0, nullptr, nullptr, nullptr, nullptr, &nc, &d.err);
     if (rc) return rc;
     const size_t off = vb::lv_slot_layout(1, cap).kp;
     return cudaMemcpy(xy, d.slot(0) + off, 8 * (size_t)nc, cudaMemcpyDeviceToHost) == cudaSuccess ? nc : VP_ERR_CUDA;
@@ -458,7 +549,7 @@ int vp_debug_brief(const uint8_t* img, int rows, int cols, const int* pattern, i
     std::vector<float> zeros(3 * (size_t)n, 0.f);
     std::vector<double> ids(n, 0.0);
     int nc = 0;
-    const int rc = attach(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, n, zeros.data(), uv, zeros.data(), ids.data(), &nc, &d.err);
+    const int rc = attach_one(d.s, 0, 0, kZeroP, kIdentityQ, img, cols, n, zeros.data(), uv, zeros.data(), ids.data(), &nc, &d.err);
     if (rc) return rc;
     const size_t off = vb::lv_slot_layout(n, vb::LV_CAP_CORNERS).wdesc;
     return cudaMemcpy(desc, d.slot(0) + off, 32 * (size_t)n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : VP_ERR_CUDA;
@@ -540,7 +631,8 @@ int vp_debug_lift(int camera_model, const double* intrinsics8, double xi, int n,
     VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpyAsync(d.slot(0) + sl.kp, uv, 8 * (size_t)n, cudaMemcpyHostToDevice, s->stream));
     VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemcpyAsync(s->d_ascratch + vb::lv_attach_layout(8, 8).status, status, sizeof(status),
                                                       cudaMemcpyHostToDevice, s->stream));
-    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, d.slot(0), s->d_pattern, 8, 8, 1, n, {}, camera_model, xi};
+    VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaMemsetAsync(s->d_jobs, 0, sizeof(long long), s->stream));  // slot 0's offset
+    vb::LvAttachLaunch L{s->d_stage, s->d_ascratch, s->d_arena, s->d_jobs, 1, s->d_pattern, 8, 8, 1, n, {}, camera_model, xi};
     std::memcpy(L.intrinsics, intrinsics8, sizeof(L.intrinsics));
     vb::launch_lv_lift(L, s->stream);
     VB_CUDA_CHECK(&d.err, VP_ERR_CUDA, cudaGetLastError());

@@ -5,7 +5,8 @@
 //   connect  brute-force Hamming matching (searchByBRIEFDes), PnP-RANSAC in float64 (one warp per hypothesis, 6-point
 //            DLT, consensus count, Gauss-Newton refit on the best consensus set), relative pose and the loop gate.
 // Every stage up to the matches is integer (or float32 where the reference is) and bit-exact; no sum uses atomics.  The
-// member / job index is the last grid dimension of every kernel.
+// member / job index is the last grid dimension of every kernel; a job finds its arena slot through a device table of
+// slot byte offsets.
 #include <cstdint>
 
 #include "camera_lift.h"
@@ -120,8 +121,8 @@ struct Intr {
 
 // One CTA per attach: exclusive scan of the row counts, then (when the corners fit) the corners in row-major order, the
 // window arrays and the header into the slot.
-__global__ void __launch_bounds__(1024, 1) lv_fast_compact_kernel(const char* stage, char* scratch, char* slot, size_t stage_stride,
-                                                               size_t scratch_stride, size_t slot_stride, int rows, int cols,
+__global__ void __launch_bounds__(1024, 1) lv_fast_compact_kernel(const char* stage, char* scratch, char* arena, const long long* slots,
+                                                               size_t stage_stride, size_t scratch_stride, int rows, int cols,
                                                                int max_window, int max_corners) {
     __shared__ int base[LV_MAX_ROWS];
     const LvAttachLayout al = lv_attach_layout(rows, cols);
@@ -129,7 +130,7 @@ __global__ void __launch_bounds__(1024, 1) lv_fast_compact_kernel(const char* st
     const LvSlotLayout sl = lv_slot_layout(max_window, max_corners);
     const char* sg = stage + blockIdx.z * stage_stride;
     char* sc = scratch + blockIdx.z * scratch_stride;
-    char* out = slot + blockIdx.z * slot_stride;
+    char* out = arena + slots[blockIdx.z];
     const int t = threadIdx.x;
     base[t] = t < rows ? reinterpret_cast<const int*>(sc + al.rowcnt)[t] : 0;
     __syncthreads();
@@ -186,15 +187,15 @@ constexpr int LIFT_THREADS = 128;
 
 // liftProjective / z of the compacted corners (computeBRIEFPoint, keyframe.cpp:108), one thread per corner, stored as float
 // like the reference's cv::Point2f.  A grid over max_corners; nothing to do when the corners overflowed.
-__global__ void __launch_bounds__(LIFT_THREADS) lv_lift_kernel(const char* scratch, char* slot, size_t scratch_stride, size_t slot_stride,
-                                                               int rows, int cols, int max_window, int max_corners, Intr intr,
-                                                               int camera_model, double xi) {
+__global__ void __launch_bounds__(LIFT_THREADS) lv_lift_kernel(const char* scratch, char* arena, const long long* slots,
+                                                               size_t scratch_stride, int rows, int cols, int max_window,
+                                                               int max_corners, Intr intr, int camera_model, double xi) {
     const LvSlotLayout sl = lv_slot_layout(max_window, max_corners);
     const int* status = reinterpret_cast<const int*>(scratch + blockIdx.z * scratch_stride + lv_attach_layout(rows, cols).status);
     if (status[1]) return;
     const int p = blockIdx.x * LIFT_THREADS + threadIdx.x;
     if (p >= status[0]) return;
-    char* out = slot + blockIdx.z * slot_stride;
+    char* out = arena + slots[blockIdx.z];
     const float* kp = reinterpret_cast<const float*>(out + sl.kp);
     float* kpn = reinterpret_cast<float*>(out + sl.kpn);
     double X, Y;
@@ -205,8 +206,8 @@ __global__ void __launch_bounds__(LIFT_THREADS) lv_lift_kernel(const char* scrat
 
 // BRIEF (DVision BRIEF::compute on the blurred image): one warp per point; blockIdx.y = 0 window points (staging uv),
 // 1 corners (slot).  Bit i = r * 32 + lane of round r; words assembled from the ballots.
-__global__ void lv_brief_kernel(const char* stage, const char* scratch, char* slot, size_t stage_stride, size_t scratch_stride,
-                                size_t slot_stride, const int* pattern, int rows, int cols, int max_window, int max_corners) {
+__global__ void lv_brief_kernel(const char* stage, const char* scratch, char* arena, const long long* slots, size_t stage_stride,
+                                size_t scratch_stride, const int* pattern, int rows, int cols, int max_window, int max_corners) {
     __shared__ int4 pat[LV_BITS];
     for (int i = threadIdx.x; i < LV_BITS; i += blockDim.x) pat[i] = reinterpret_cast<const int4*>(pattern)[i];
     __syncthreads();
@@ -214,7 +215,7 @@ __global__ void lv_brief_kernel(const char* stage, const char* scratch, char* sl
     const LvSlotLayout sl = lv_slot_layout(max_window, max_corners);
     const char* sg = stage + blockIdx.z * stage_stride;
     const char* sc = scratch + blockIdx.z * scratch_stride;
-    char* out = slot + blockIdx.z * slot_stride;
+    char* out = arena + slots[blockIdx.z];
     const int* status = reinterpret_cast<const int*>(sc + al.status);
     if (status[1]) return;
     const bool win = blockIdx.y == 0;
@@ -681,25 +682,25 @@ void launch_lv_scatter(char* arena, const char* staged, int n_kf, int max_window
 void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s) {
     Intr in;
     for (int i = 0; i < 8; i++) in.v[i] = L.intrinsics[i];
-    lv_lift_kernel<<<dim3((L.max_corners + LIFT_THREADS - 1) / LIFT_THREADS, 1, 1), LIFT_THREADS, 0, s>>>(
-        L.scratch, L.slot, lv_attach_layout(L.rows, L.cols).total, lv_slot_layout(L.max_window, L.max_corners).total, L.rows, L.cols,
-        L.max_window, L.max_corners, in, L.camera_model, L.xi);
+    lv_lift_kernel<<<dim3((L.max_corners + LIFT_THREADS - 1) / LIFT_THREADS, 1, L.n_jobs), LIFT_THREADS, 0, s>>>(
+        L.scratch, L.arena, L.slots, lv_attach_layout(L.rows, L.cols).total, L.rows, L.cols, L.max_window, L.max_corners, in,
+        L.camera_model, L.xi);
 }
 
 int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev) {
     const size_t stage_stride = lv_stage_layout(L.rows, L.cols, L.max_window).total, scratch_stride = lv_attach_layout(L.rows, L.cols).total;
-    const size_t slot_stride = lv_slot_layout(L.max_window, L.max_corners).total;
+    const int z = L.n_jobs;
     if (ev) cudaEventRecord(ev[0], s);
-    lv_blur_kernel<<<dim3((L.cols + BLUR_TX - 1) / BLUR_TX, (L.rows + BLUR_TY - 1) / BLUR_TY, 1), dim3(BLUR_TX, BLUR_TY), 0, s>>>(
+    lv_blur_kernel<<<dim3((L.cols + BLUR_TX - 1) / BLUR_TX, (L.rows + BLUR_TY - 1) / BLUR_TY, z), dim3(BLUR_TX, BLUR_TY), 0, s>>>(
         L.stage, L.scratch, stage_stride, scratch_stride, L.rows, L.cols);
     if (ev) cudaEventRecord(ev[1], s);
-    lv_fast_score_kernel<<<dim3((L.cols + 127) / 128, L.rows, 1), 128, 0, s>>>(L.stage, L.scratch, stage_stride, scratch_stride, L.rows, L.cols);
-    lv_fast_nms_kernel<<<dim3(1, L.rows, 1), 256, 0, s>>>(L.scratch, scratch_stride, L.rows, L.cols);
-    lv_fast_compact_kernel<<<dim3(1, 1, 1), 1024, 0, s>>>(L.stage, L.scratch, L.slot, stage_stride, scratch_stride, slot_stride, L.rows,
+    lv_fast_score_kernel<<<dim3((L.cols + 127) / 128, L.rows, z), 128, 0, s>>>(L.stage, L.scratch, stage_stride, scratch_stride, L.rows, L.cols);
+    lv_fast_nms_kernel<<<dim3(1, L.rows, z), 256, 0, s>>>(L.scratch, scratch_stride, L.rows, L.cols);
+    lv_fast_compact_kernel<<<dim3(1, 1, z), 1024, 0, s>>>(L.stage, L.scratch, L.arena, L.slots, stage_stride, scratch_stride, L.rows,
                                                            L.cols, L.max_window, L.max_corners);
     launch_lv_lift(L, s);
     if (ev) cudaEventRecord(ev[2], s);
-    lv_brief_kernel<<<dim3(64, 2, 1), 256, 0, s>>>(L.stage, L.scratch, L.slot, stage_stride, scratch_stride, slot_stride, L.pattern, L.rows,
+    lv_brief_kernel<<<dim3(64, 2, z), 256, 0, s>>>(L.stage, L.scratch, L.arena, L.slots, stage_stride, scratch_stride, L.pattern, L.rows,
                                                     L.cols, L.max_window, L.max_corners);
     if (ev) cudaEventRecord(ev[3], s);
     return 6;

@@ -7,13 +7,16 @@
 
 namespace vb {
 
-// One key frame: staging block (lv_stage_layout) -> scratch (lv_attach_layout) -> slot (lv_slot_layout).  The slot is
-// written only when the corner count fits max_corners; scratch status = {corner count, overflow}.
+// n_jobs key frames, job j: staging block j (lv_stage_layout) -> scratch j (lv_attach_layout) -> the arena slot at byte
+// offset slots[j] (lv_slot_layout).  Blocks and scratches lie at their layout's total stride.  A slot is written only
+// when its corner count fits max_corners; scratch status = {corner count, overflow}.
 struct LvAttachLaunch {
     const char* stage;
     char* scratch;
-    char* slot;
-    const int* pattern;  // device, 256 x (x1, y1, x2, y2)
+    char* arena;
+    const long long* slots;  // device, n_jobs slot byte offsets into the arena
+    int n_jobs;
+    const int* pattern;      // device, 256 x (x1, y1, x2, y2)
     int rows, cols, max_window, max_corners;
     double intrinsics[8];  // in the order of camera_model (camera_lift.h)
     int camera_model;      // CAM_PINHOLE, CAM_MEI or CAM_KANNALA_BRANDT
@@ -22,7 +25,7 @@ struct LvAttachLaunch {
 // ev (may be NULL): 4 events recorded before the blur, the FAST stage (FAST, compaction and the corner lift), BRIEF and
 // after BRIEF.  Returns launches.
 int launch_lv_attach(const LvAttachLaunch& L, cudaStream_t s, cudaEvent_t* ev);
-// The corner lift alone: the status and the corners kp already in scratch and slot.
+// The corner lift alone: the status and the corners kp already in scratch and slots.
 void launch_lv_lift(const LvAttachLaunch& L, cudaStream_t s);
 
 // Loaded key frames into their slots (vp_load): staged (device) holds n_kf jobs and blocks as lv_load_layout defines them;

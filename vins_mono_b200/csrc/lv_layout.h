@@ -75,6 +75,9 @@ LV_LAYOUT_FN LvStageLayout lv_stage_layout(int rows, int cols, int max_window) {
     o.total = o.id + lv_align16(8 * w);
     return o;
 }
+// the packed stage of one attach call (one host-to-device copy): per job its slot's byte offset in the arena (long long),
+// padded to 16 bytes | per job a staging block at lv_stage_layout's total stride
+LV_LAYOUT_FN size_t lv_attach_jobs_bytes(int n_jobs) { return lv_align16(8 * (size_t)n_jobs); }
 
 // ---- staging of the key frames one vp_load puts into their slots (one host-to-device copy), in bytes: per key frame a
 //      job (slot byte offset in the arena, block byte offset in the staging buffer: 2 x long long) | per key frame a

@@ -6,7 +6,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._abi import Batch, Handle, LoopConfig, LoopResult, PoseGraphConfig, VinsError, check, f64, load_library, ptr
+from ._abi import AttachJob, Batch, Handle, LoopConfig, LoopResult, PoseGraphConfig, VinsError, check, f64, load_library, ptr
 
 PoseGraphError = VinsError
 VP_ERR_CAPACITY = -4
@@ -153,6 +153,43 @@ class PoseGraphBatch(Batch):
         for m in self.members:
             m._loop_cap = cfg.max_window
         self._check(self.lib.vp_batch_loop_enable_camera(self.h, C.byref(cfg), int(camera_model), float(xi)))
+
+    def attach_keyframes(self, jobs):
+        """Several key frames, of any members, attached in one launch chain.  jobs: tuples (member, index, vio_P,
+        vio_Q_wxyz, image, point_3d, point_uv, point_norm, point_id) as PoseGraph.attach_keyframe takes them; image is a
+        uint8 array or a CUDA tensor on the batch's device (rows x cols, unit column stride), read once torch's current
+        stream on that device has finished the work queued before the call.  Returns (n_corners, status)
+        per job: status VP_ERR_CAPACITY = -4 for a job with more corners than max_corners, whose slot is left as it was
+        while the other jobs are written.  Any other error raises and attaches nothing."""
+        arr, keep, devices = (AttachJob * len(jobs))(), [], set()
+        for j, (member, index, P, Q, image, p3d, uv, norm, pid) in enumerate(jobs):
+            a = arr[j]
+            a.member, a.index = int(member), int(index)
+            P, Q = f64(P), f64(Q)
+            p3 = np.ascontiguousarray(p3d, np.float32).reshape(-1, 3)
+            pts = [p3, np.ascontiguousarray(uv, np.float32).reshape(-1, 2), np.ascontiguousarray(norm, np.float32).reshape(-1, 2),
+                   np.ascontiguousarray(pid, np.float64).reshape(-1)]
+            if getattr(image, "is_cuda", False):
+                img = image
+                if img.element_size() != 1 or img.dim() != 2 or img.stride(1) != 1:
+                    raise ValueError("a device image is a 2-D uint8 CUDA tensor with unit column stride")
+                a.img, a.row_stride, a.img_on_device = img.data_ptr(), img.stride(0), 1
+                devices.add(img.device)
+            else:
+                img = np.ascontiguousarray(image, np.uint8)
+                a.img, a.row_stride, a.img_on_device = img.ctypes.data, img.strides[0], 0
+            a.vio_P3, a.vio_Qwxyz = P.ctypes.data, Q.ctypes.data
+            a.n = len(p3)
+            a.point_3d, a.point_uv, a.point_norm, a.point_id = (v.ctypes.data for v in pts)
+            keep += [P, Q, img, *pts]
+        if devices:  # the library copies device images on its own stream, which does not wait for torch's
+            import torch
+            for d in devices:
+                torch.cuda.current_stream(d).synchronize()
+        nc, st = np.zeros(len(jobs), np.int32), np.zeros(len(jobs), np.int32)
+        rc = self.lib.vp_batch_attach_keyframes(self.h, len(jobs), arr, ptr(nc), ptr(st))
+        self._check(0 if rc == VP_ERR_CAPACITY and (st == VP_ERR_CAPACITY).any() else rc)
+        return nc, st
 
     def find_connection(self, cur, old):
         """One launch chain for every member k with cur[k] >= 0; returns a list (None for skipped members)."""
